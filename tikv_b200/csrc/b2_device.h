@@ -27,7 +27,7 @@
 // Decoders that only the general (dirty-data / v1 / odd-row) paths call: out of line when jit.cu sets B2_COLD_OUTLINE (plans
 // with the rarer scalar functions, whose unrolled evaluators make NVRTC slow), inlined everywhere else: the scan kernel's
 // register allocation is sensitive to it.  The clean-entry paths have their own branch-free decoders.
-#if defined(B2_COLD_OUTLINE) && !defined(B2_NO_COLD_OUTLINE) && defined(__CUDACC__)
+#if defined(B2_COLD_OUTLINE) && defined(__CUDACC__)
 #define B2_COLD __device__ __noinline__
 #else
 #define B2_COLD B2_HD

@@ -107,9 +107,22 @@ struct BufPool {
 BufPool& dev_pool() { static BufPool p(false, 24ull << 30); return p; }
 BufPool& host_pool() { static BufPool p(true, 8ull << 30); return p; }
 
-struct DevBuf {  // growable device allocation (pooled)
+// A block taken from `Pool` and owned: it goes back to the pool when the buffer is destroyed or released, moving leaves the
+// source empty.  The pool tags a returned block with the current device, so that device must be current then.
+template <BufPool& (*Pool)()>
+struct PooledBuf {
   void* p = nullptr;
   size_t cap = 0;
+  PooledBuf() = default;
+  PooledBuf(PooledBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  PooledBuf& operator=(PooledBuf&& o) noexcept {
+    if (this != &o) { release(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+    return *this;
+  }
+  ~PooledBuf() { release(); }
+  void release() { if (p) Pool().put(p, cap); p = nullptr; cap = 0; }
+};
+struct DevBuf : PooledBuf<dev_pool> {  // growable device allocation
   cudaError_t reserve(size_t n) {
     if (n <= cap) return cudaSuccess;
     if (p) cudaDeviceSynchronize();  // growing: in-flight work may still touch the old block before it goes back to the pool
@@ -123,17 +136,13 @@ struct DevBuf {  // growable device allocation (pooled)
     release();
     return dev_pool().get(n, &p, &cap);
   }
-  void release() { if (p) dev_pool().put(p, cap); p = nullptr; cap = 0; }
 };
-struct HostBuf {  // growable pinned host allocation (pooled)
-  void* p = nullptr;
-  size_t cap = 0;
+struct HostBuf : PooledBuf<host_pool> {  // growable pinned host allocation
   cudaError_t reserve(size_t n) {
     if (n <= cap) return cudaSuccess;
     release();
     return host_pool().get(n, &p, &cap);
   }
-  void release() { if (p) host_pool().put(p, cap); p = nullptr; cap = 0; }
 };
 
 struct SrcBlock {  // caller's block descriptor + sizes
@@ -315,36 +324,38 @@ struct b2_exec {
     return status;
   }
 
+  // The buffer members are destroyed after this body has run, so the device is still current (BufPool::put tags a block
+  // with it) and both streams are drained when their blocks go back to the pool.
   ~b2_exec() {
     cudaSetDevice(device);
     if (stream) cudaStreamSynchronize(stream);
     if (copy_stream) { cudaStreamSynchronize(copy_stream); cudaStreamDestroy(copy_stream); }
     for (auto& s : slots) {
-      s.keys.release(); s.koff.release(); s.vals.release(); s.voff.release();
       if (s.ready) cudaEventDestroy(s.ready);
       if (s.free_ev) cudaEventDestroy(s.free_ev);
     }
     for (auto& e : kev) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
-    for (DevBuf* b : {&tn_work, &tn_lists, &tn_counts, &tn_pair, &tn_pair_cnt, &tn_tmp, &tn_tmp_cnt, &tn_blk_pay, &tn_blk_null, &tn_run_pay, &tn_run_null, &tn_tmp_pay, &tn_tmp_null, &tn_bitmap}) b->release();
-    for (DevBuf* b : {&ctr_buf, &status_buf, &out_data, &out_bitmap, &dflt_views, &dflt_store, &tbl_keys, &tbl_occ, &tbl_acc, &tbl_gkeys, &tbl_ready, &grp_keys, &grp_null, &grp_acc, &res_ptrs, &range_rows, &range_rows_prev, &slow_list, &slow_cnt, &const_pool, &rev_data, &rev_bitmap, &enc_cols, &enc_counts, &enc_out, &enc_lens, &enc_offs, &enc_tmp, &tn_lvl_a, &tn_lvl_a_cnt, &tn_lvl_b, &tn_lvl_b_cnt}) b->release();
-    enc_host.release();
-    for (auto& b : res_cols) b.release();
-    for (auto& b : res_bitmaps) b.release();
-    h_out.release(); h_ctr.release(); h_raw.release(); h_raw_out.release();
-    raw_state.release(); raw_sums.release();
-    for (RawOut& r : raw_outs) { r.offs.release(); r.heap.release(); }
     if (own_stream && stream) cudaStreamDestroy(stream);
+  }
+  // the handle's streams: kernels run on the caller's stream (cfg->cuda_stream) or an own one, block staging on an own one
+  cudaError_t open_streams(const b2_exec_config* cfg) {
+    if (cfg && cfg->cuda_stream) stream = (cudaStream_t)cfg->cuda_stream;
+    else {
+      cudaError_t e = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
+      if (e != cudaSuccess) return e;
+      own_stream = true;
+    }
+    return cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking);
   }
 
   Counters* ctr() { return (Counters*)ctr_buf.p; }
 
   // ---- plan-specialised kernel (jit.cu): used as soon as its compilation has finished, the generic kernel until then ----
-  enum { JIT_AUTO = 0, JIT_SYNC = 1, JIT_OFF = 2 };
-  int jit_mode = JIT_AUTO;
+  int jit_mode = B2_JIT_AUTO;
   bool jit_started = false;
   std::shared_future<JitKernel*> jit_fut;
   void jit_start() {
-    if (jit_started || jit_mode == JIT_OFF || cp.dev.mode == PM_CHECKSUM || !jit_available()) return;
+    if (jit_started || jit_mode == B2_JIT_OFF || cp.dev.mode == PM_CHECKSUM || !jit_available()) return;
     jit_fut = jit_get(device, cp.dev);
     jit_started = true;
   }
@@ -563,7 +574,6 @@ struct b2_exec {
       if (e == cudaSuccess) e = cudaMemcpyAsync(res.data(), d_res.p, res.size() * 4, cudaMemcpyDeviceToHost, stream);
       if (e == cudaSuccess) e = cudaMemcpyAsync(unit_ok.data(), d_ok.p, unit_ok.size() * 4, cudaMemcpyDeviceToHost, stream);
       if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-      d_views.release(); d_flat.release(); d_offs.release(); d_res.release(); d_ok.release();
       if (e != cudaSuccess) return fail(B2_ERR_CUDA, std::string("range bounds search: ") + cudaGetErrorString(e));
     }
     for (uint32_t r = first_live_range; r < nr; ++r)
@@ -606,17 +616,13 @@ struct b2_exec {
     CUDA_TRY(cudaMemcpyAsync(s->vals.p, sb.c.vals, sb.val_bytes, cudaMemcpyHostToDevice, copy_stream));
     // the readable bytes past the heaps (word-wide loads of the last entries land there) are zero, as the padding contract of
     // device-resident blocks has them: nothing may depend on what an earlier request left in a recycled buffer
-    static const bool pad_zero = getenv("B2_NO_STAGE_PAD") == nullptr;
-    if (pad_zero) {
-      CUDA_TRY(cudaMemsetAsync((uint8_t*)s->keys.p + sb.key_bytes, 0, kb - sb.key_bytes, copy_stream));
-      CUDA_TRY(cudaMemsetAsync((uint8_t*)s->vals.p + sb.val_bytes, 0, vb - sb.val_bytes, copy_stream));
-    }
+    CUDA_TRY(cudaMemsetAsync((uint8_t*)s->keys.p + sb.key_bytes, 0, kb - sb.key_bytes, copy_stream));
+    CUDA_TRY(cudaMemsetAsync((uint8_t*)s->vals.p + sb.val_bytes, 0, vb - sb.val_bytes, copy_stream));
     CUDA_TRY(cudaMemcpyAsync(s->koff.p, sb.c.key_offs, ob, cudaMemcpyHostToDevice, copy_stream));
     CUDA_TRY(cudaMemcpyAsync(s->voff.p, sb.c.val_offs, ob, cudaMemcpyHostToDevice, copy_stream));
     CUDA_TRY(cudaEventRecord(s->ready, copy_stream));
     s->block = (int)bi;
     s->done = false;
-    stats.default_lookups += 0;
     h2d_bytes += sb.key_bytes + sb.val_bytes + 2 * ob;
     *out = s;
     return B2_OK;
@@ -727,21 +733,15 @@ struct b2_exec {
       a->stage_key_cap = cap(sb.key_bytes, 130); a->stage_val_cap = cap(sb.val_bytes, 130);
       total = a->stage_off + scan_stage_bytes(a->stage_key_cap, a->stage_val_cap);
     }
-    if (!use_staging || total > 200 * 1024) { a->staging = 0; a->stage_key_cap = a->stage_val_cap = 0; return mode_bytes; }
+    if (total > 200 * 1024) { a->staging = 0; a->stage_key_cap = a->stage_val_cap = 0; return mode_bytes; }
     a->staging = 1;
     return total;
   }
-  bool use_staging = true;
   // ---- order-free pipelines: the lean kernel (fast_kernel.cuh) over a unit, then scan_body in list mode over the runs it
   // handed over (their first entries, appended on the device; the count never visits the host) ----
   DevBuf slow_list, slow_cnt;
   DevBuf const_pool;  // bytes constants of the plan (CompiledPlan::pool)
-  bool use_fast_kernel = getenv("B2_NO_FAST_KERNEL") == nullptr;
-  bool fast_kernel_covers() const {
-    if (!use_fast_kernel) return false;
-    if (cp.dev.mode == PM_CHECKSUM) return true;
-    return plan_has_fast_kernel(cp.dev);
-  }
+  bool fast_kernel_covers() const { return cp.dev.mode == PM_CHECKSUM || plan_has_fast_kernel(cp.dev); }
   // `a`: the unit's arguments (c_lo / c_hi set, mode pointers set).  general_smem_mode / fast_smem_mode: bytes of mode state
   // in front of the stages; fast_slots: CTA table slots of the lean aggregation kernel.
   int launch_unit(const ScanArgs& a0, const Unit& u, bool fast, size_t general_smem_mode, size_t fast_smem_mode, uint32_t fast_slots, int* general_grid_out,
@@ -750,10 +750,10 @@ struct b2_exec {
     if (!fast) {
       ScanArgs a = a0;
       size_t tot = setup_staging(&a, wblocks[u.block_idx], general_smem_mode);
-      int grid = cp.dev.mode == PM_CHECKSUM ? scan_max_grid(PM_CHECKSUM, tot) : scan_grid_for(mode, tot);
+      int grid = scan_grid_for(mode, tot);
       if (general_grid_out && *general_grid_out > 0) grid = std::min(grid, *general_grid_out);
       kernel_begin();
-      CUDA_TRY(cp.dev.mode == PM_CHECKSUM ? launch_scan(cp.dev, a, grid, tot, stream) : scan_launch(a, grid, tot));
+      CUDA_TRY(scan_launch(a, grid, tot));
       kernel_end();
       if (general_grid_out) *general_grid_out = grid;
       if (fast_grid_out) *fast_grid_out = 0;
@@ -766,7 +766,7 @@ struct b2_exec {
     f.slow_list = (unsigned int*)slow_list.p; f.slow_count = (unsigned int*)slow_cnt.p;
     f.smem_slots = fast_slots;
     size_t ftot = setup_staging(&f, wblocks[u.block_idx], fast_smem_mode);
-    const JitKernel* jk = cp.dev.mode == PM_CHECKSUM ? nullptr : jit_ready();
+    const JitKernel* jk = jit_ready();
     if (jk && !jk->fn_fast) jk = nullptr;
     int fgrid = jk ? jit_max_blocks_per_sm(jk, ftot, true) * scan_num_sms() : fast_max_grid(cp.dev.mode, ftot);
     if (fast_grid_out && *fast_grid_out > 0) fgrid = std::min(fgrid, *fast_grid_out);
@@ -779,27 +779,24 @@ struct b2_exec {
     }
     ScanArgs g = a0;
     size_t gtot = general_smem_mode;
-    int ggrid;
     if (fast) {
       g.slow_list = f.slow_list; g.slow_count = f.slow_count; g.list_mode = 1;
       g.staging = 0; g.stage_off = 0; g.stage_key_cap = g.stage_val_cap = 0;
-      ggrid = cp.dev.mode == PM_CHECKSUM ? scan_max_grid(PM_CHECKSUM, gtot) : scan_grid_for(mode, gtot);
     } else {
       gtot = setup_staging(&g, wblocks[u.block_idx], general_smem_mode);
-      ggrid = cp.dev.mode == PM_CHECKSUM ? scan_max_grid(PM_CHECKSUM, gtot) : scan_grid_for(mode, gtot);
     }
+    int ggrid = scan_grid_for(mode, gtot);
     if (general_grid_out && *general_grid_out > 0) ggrid = std::min(ggrid, *general_grid_out);
     if (cp.dev.mode == PM_TOPN && fast) {  // the two kernels leave their per-CTA lists side by side
       g.topn.items = a0.topn.items + (size_t)fgrid * a0.topn.stride; g.topn.counts = a0.topn.counts + fgrid;
     }
-    CUDA_TRY(cp.dev.mode == PM_CHECKSUM ? launch_scan(cp.dev, g, ggrid, gtot, stream) : scan_launch(g, ggrid, gtot));
+    CUDA_TRY(scan_launch(g, ggrid, gtot));
     kernel_end();
     stats.kernel_launches += fast ? 1 : 0;
     if (general_grid_out) *general_grid_out = ggrid;
     if (fast_grid_out) *fast_grid_out = fast ? fgrid : 0;
     return B2_OK;
   }
-  bool use_fast_front = getenv("B2_NO_FAST_FRONT") == nullptr;  // debug switch: general front end only
 
   ScanArgs base_args(const Unit& u, const BlockView& v) {
     ScanArgs a;
@@ -810,7 +807,7 @@ struct b2_exec {
     a.entry_base = wblocks[u.block_idx].entry_base;
     a.ctr = ctr();
     a.read_ts = cp.dev.read_ts; a.isolation = cp.dev.isolation;
-    a.fast_ok = use_fast_front ? u.fast_ok : 0;
+    a.fast_ok = u.fast_ok;
     a.desc = cp.desc ? 1u : 0u;
     memcpy(a.imms, cp.imms, sizeof(a.imms));
     a.limit = cp.dev.limit;
@@ -821,8 +818,65 @@ struct b2_exec {
   // ---- PM_SCAN: up to `scan_rows` CF_WRITE entries per call, appended in key order into one set of columns ----
   // One pass = one launch per (range, block) unit touched; launches chain on the stream through the device-side
   // row counter (out_rows -> out_base), so there is a single host sync per batch.
+  // output columns (8-byte cells) for `rows` rows in `data` / `bitmap`, their non-NULL bitmaps set to ones
+  int reserve_out(DevBuf* data, DevBuf* bitmap, uint64_t* cap_now, uint64_t rows) {
+    const size_t n_out = cp.dev.n_out;
+    const uint64_t cap = std::max<uint64_t>(64, (rows + 63) & ~63ull);
+    if (cap > *cap_now) {
+      CUDA_TRY(cudaStreamSynchronize(stream));
+      CUDA_TRY(data->reserve(cap * 8 * n_out)); CUDA_TRY(bitmap->reserve(cap / 8 * n_out));
+      *cap_now = cap;
+    }
+    CUDA_TRY(cudaMemsetAsync(bitmap->p, 0xff, *cap_now / 8 * n_out, stream));
+    return B2_OK;
+  }
+  // one launch over the entries [c_lo, c_hi) of unit `u`, appending to the output columns; the walks of the chunk's last
+  // runs stop at e_hi
+  int scan_chunk(const Unit& u, uint32_t c_lo, uint32_t c_hi, uint32_t e_hi) {
+    const uint32_t n_tiles = (c_hi - c_lo + TILE - 1) / TILE;
+    CUDA_TRY(status_buf.reserve_on(stream, ((size_t)n_tiles + 1) * 8));
+    CUDA_TRY(cudaMemsetAsync(status_buf.p, 0, ((size_t)n_tiles + 1) * 8, stream));
+    BlockView v;
+    int rc = acquire_block(u.block_idx, &v);
+    if (rc) return rc;
+    ScanArgs a = base_args(u, v);
+    a.c_lo = c_lo; a.c_hi = c_hi; a.e_hi = e_hi;
+    a.tile_status = (unsigned long long*)status_buf.p;
+    a.out_data = (unsigned long long*)out_data.p; a.out_bitmap = (unsigned long long*)out_bitmap.p;
+    a.out_cap = out_cap;
+    const size_t smem = setup_staging(&a, wblocks[u.block_idx], scan_out_stage_bytes());
+    a.out_stage_off = 0;
+    const int grid = scan_grid_for(scan_kernel_mode(cp.dev), smem);
+    kernel_begin();
+    CUDA_TRY(scan_launch(a, grid, smem));
+    kernel_end();
+    if (cp.dev.n_raw) { rc = raw_materialise(a, c_hi - c_lo); if (rc) return rc; }
+    release_block(u.block_idx);
+    stats.num_iterations++;
+    return B2_OK;
+  }
+  // BatchLimitExecutor (limit_executor.rs:55-80): a plain scan needs at most `remaining` more rows, so do not read far
+  // past them; with a selection in between the batch size is the caller's.  Returns the batch's entry budget.
+  uint64_t begin_scan_batch(uint64_t scan_rows) {
+    cols.clear();
+    uint64_t budget = std::max<uint64_t>(1, std::min<uint64_t>(scan_rows, 1ull << 31));
+    if (cp.scan_limit == ~0ull) return budget;
+    if (limit_remaining == ~0ull) limit_remaining = cp.scan_limit;
+    if (limit_remaining == 0) drained = true;
+    if (cp.dev.n_conds == 0) budget = std::min<uint64_t>(budget, std::max<uint64_t>(4096, limit_remaining * 2));
+    return budget;
+  }
+  // the rows of the batch that the Limit still takes
+  uint64_t limit_take(uint64_t produced) {
+    if (cp.scan_limit == ~0ull) return produced;
+    if (produced < limit_remaining) { limit_remaining -= produced; return produced; }
+    produced = limit_remaining;
+    limit_remaining = 0;
+    drained = true;
+    return produced;
+  }
+
   int run_scan_pass(uint64_t budget, uint64_t stop_before, bool* hit_lock_range, uint32_t* lock_range, Counters* c) {
-    size_t n_out = cp.dev.n_out;
     // capacity = entries this pass may cover
     uint64_t need = 0, left = budget;
     {
@@ -834,13 +888,8 @@ struct b2_exec {
         ++u; e = 0;
       }
     }
-    uint64_t cap = std::max<uint64_t>(64, (need + 63) & ~63ull);
-    if (cap > out_cap) {
-      CUDA_TRY(cudaStreamSynchronize(stream));
-      CUDA_TRY(out_data.reserve(cap * 8 * n_out)); CUDA_TRY(out_bitmap.reserve(cap / 8 * n_out));
-      out_cap = cap;
-    }
-    CUDA_TRY(cudaMemsetAsync(out_bitmap.p, 0xff, out_cap / 8 * n_out, stream));
+    int rc = reserve_out(&out_data, &out_bitmap, &out_cap, need);
+    if (rc) return rc;
     if (cp.dev.n_raw) {
       // every byte a cell reference of this pass can point at: the value heaps of the blocks it touches (+ CF_DEFAULT)
       uint64_t vb = 0;
@@ -855,12 +904,9 @@ struct b2_exec {
         for (const SrcBlock& d : dblocks) vb += d.val_bytes;
       }
       CUDA_TRY(cudaStreamSynchronize(stream));
-      int rrc = raw_prepare(out_cap, vb);
-      if (rrc) return rrc;
+      rc = raw_prepare(out_cap, vb);
+      if (rc) return rc;
     }
-    Counters z;
-    memset(&z, 0, sizeof(z));
-    z.err = ~0ull; z.first_row = ~0ull;
     // keep request-level statistics, reset the per-batch row counters
     CUDA_TRY(cudaMemsetAsync(&ctr()->out_rows, 0, 8, stream));
     CUDA_TRY(cudaMemsetAsync(&ctr()->out_base, 0, 8, stream));
@@ -877,44 +923,12 @@ struct b2_exec {
         stop_here = true;
       }
       if (c_hi > c_lo) {
-        uint32_t n_tiles = (c_hi - c_lo + TILE - 1) / TILE;
-        CUDA_TRY(status_buf.reserve_on(stream, ((size_t)n_tiles + 1) * 8));
-        CUDA_TRY(cudaMemsetAsync(status_buf.p, 0, ((size_t)n_tiles + 1) * 8, stream));
-        BlockView v;
-        int rc = acquire_block(u.block_idx, &v);
+        // (the failing entry is a run start: nothing before it can reach past it)
+        rc = scan_chunk(u, c_lo, c_hi, stop_here ? c_hi : u.e_hi);
         if (rc) return rc;
-        ScanArgs a = base_args(u, v);
-        a.c_lo = c_lo; a.c_hi = c_hi;
-        if (stop_here) a.e_hi = c_hi;  // the failing entry is a run start: nothing before it can reach past it
-        a.tile_status = (unsigned long long*)status_buf.p;
-        a.out_data = (unsigned long long*)out_data.p; a.out_bitmap = (unsigned long long*)out_bitmap.p;
-        a.out_cap = out_cap;
-        size_t smem = setup_staging(&a, wblocks[u.block_idx], scan_out_stage_bytes());
-        a.out_stage_off = 0;
-        if (getenv("B2_TRACE") && !trace_done) { trace_buf.reserve(128 * 8 * 8); cudaMemsetAsync(trace_buf.p, 0, 128 * 8 * 8, stream); a.trace = (unsigned long long*)trace_buf.p; }
-        scan_grid = scan_grid_for(scan_kernel_mode(cp.dev), smem);
-        kernel_begin();
-        CUDA_TRY(scan_launch(a, scan_grid, smem));
-        kernel_end();
-        if (cp.dev.n_raw) { int rrc = raw_materialise(a, c_hi - c_lo); if (rrc) return rrc; }
         CUDA_TRY(cudaMemcpyAsync(&ctr()->out_base, &ctr()->out_rows, 8, cudaMemcpyDeviceToDevice, stream));
-        if (a.trace && !trace_done) {
-          trace_done = true;
-          std::vector<unsigned long long> t(128 * 8);
-          cudaStreamSynchronize(stream);
-          cudaMemcpy(t.data(), trace_buf.p, t.size() * 8, cudaMemcpyDeviceToHost);
-          fprintf(stderr, "B2_TRACE tile: wait_full decode+pred sync1 out_decode obuf_wait out_store tail | cycle (SM clocks, CTA 0 thread 0)\n");
-          for (int i = 1; i < 40; ++i) {
-            unsigned long long* r = &t[i * 8];
-            if (!r[6]) break;
-            fprintf(stderr, "B2_TRACE %3d: %7lld %7lld %7lld %7lld %7lld %7lld %7lld | %7lld\n", i, (long long)(r[5] - r[4]), (long long)(r[0] - r[5]), (long long)(r[1] - r[0]),
-                    (long long)(r[2] - r[1]), (long long)(r[3] - r[2]), (long long)(r[7] - r[3]), (long long)(r[6] - r[7]), (long long)(r[6] - t[(i - 1) * 8 + 6]));
-          }
-        }
-        release_block(u.block_idx);
         entries_scanned += c_hi - c_lo;
         budget -= c_hi - c_lo;
-        stats.num_iterations++;
       }
       cur_entry = c_hi;
       if (stop_here) break;
@@ -930,15 +944,9 @@ struct b2_exec {
   }
 
   int next_scan_batch(uint64_t scan_rows, b2_batch* out) {
-    cols.clear();
-    uint64_t budget = std::max<uint64_t>(1, std::min<uint64_t>(scan_rows, 1ull << 31));
-    uint64_t produced = 0;
-    // BatchLimitExecutor (limit_executor.rs:55-80): a plain scan needs at most `remaining` more rows, so do not read far
-    // past them; with a selection in between the batch size is the caller's
+    const uint64_t budget = begin_scan_batch(scan_rows);
     const bool limited = cp.scan_limit != ~0ull;
-    if (limited && limit_remaining == ~0ull) limit_remaining = cp.scan_limit;
-    if (limited && limit_remaining == 0) drained = true;
-    if (limited && cp.dev.n_conds == 0) budget = std::min<uint64_t>(budget, std::max<uint64_t>(4096, limit_remaining * 2));
+    uint64_t produced = 0;
     while (!drained && !failed && produced == 0) {
       if (cur_unit >= units.size()) { drained = true; break; }
       size_t save_unit = cur_unit; uint32_t save_entry = cur_entry; uint64_t save_scanned = entries_scanned;
@@ -978,10 +986,7 @@ struct b2_exec {
         break;
       }
     }
-    if (limited) {
-      if (produced < limit_remaining) limit_remaining -= produced;
-      else { produced = limit_remaining; limit_remaining = 0; drained = true; }
-    }
+    produced = limit_take(produced);
     if (!failed && cur_unit >= units.size()) {
       drained = true;
       if (!(limited && limit_remaining == 0)) check_trailing_lock();
@@ -1000,38 +1005,15 @@ struct b2_exec {
   DevBuf rev_data, rev_bitmap;
   uint64_t rev_cap = 0;
   int run_desc_chunk(const Unit& u, uint32_t c_lo, uint32_t c_hi, Counters* c) {
-    const size_t n_out = cp.dev.n_out;
-    const uint64_t cap = std::max<uint64_t>(64, ((uint64_t)(c_hi - c_lo) + 63) & ~63ull);
-    if (cap > out_cap) {
-      CUDA_TRY(cudaStreamSynchronize(stream));
-      CUDA_TRY(out_data.reserve(cap * 8 * n_out)); CUDA_TRY(out_bitmap.reserve(cap / 8 * n_out));
-      out_cap = cap;
-    }
-    CUDA_TRY(cudaMemsetAsync(out_bitmap.p, 0xff, out_cap / 8 * n_out, stream));
+    int rc = reserve_out(&out_data, &out_bitmap, &out_cap, c_hi - c_lo);
+    if (rc) return rc;
     Counters z;
     memset(&z, 0, sizeof(z));
     z.err = ~0ull; z.first_row = ~0ull;
     // per-chunk counters; request-level statistics are carried on the host (desc_stats)
     CUDA_TRY(cudaMemcpyAsync(ctr_buf.p, &z, sizeof(z), cudaMemcpyHostToDevice, stream));
-    const uint32_t n_tiles = (c_hi - c_lo + TILE - 1) / TILE;
-    CUDA_TRY(status_buf.reserve_on(stream, ((size_t)n_tiles + 1) * 8));
-    CUDA_TRY(cudaMemsetAsync(status_buf.p, 0, ((size_t)n_tiles + 1) * 8, stream));
-    BlockView v;
-    int rc = acquire_block(u.block_idx, &v);
+    rc = scan_chunk(u, c_lo, c_hi, u.e_hi);
     if (rc) return rc;
-    ScanArgs a = base_args(u, v);
-    a.c_lo = c_lo; a.c_hi = c_hi;
-    a.tile_status = (unsigned long long*)status_buf.p;
-    a.out_data = (unsigned long long*)out_data.p; a.out_bitmap = (unsigned long long*)out_bitmap.p;
-    a.out_cap = out_cap;
-    size_t smem = setup_staging(&a, wblocks[u.block_idx], scan_out_stage_bytes());
-    a.out_stage_off = 0;
-    scan_grid = scan_grid_for(scan_kernel_mode(cp.dev), smem);
-    kernel_begin();
-    CUDA_TRY(scan_launch(a, scan_grid, smem));
-    kernel_end();
-    release_block(u.block_idx);
-    stats.num_iterations++;
     return read_counters(c);
   }
   Counters desc_stats{};  // request-level sums of the per-chunk counters
@@ -1042,13 +1024,9 @@ struct b2_exec {
     first_row_seen = std::min<uint64_t>(first_row_seen, c.first_row);
   }
   int next_scan_batch_desc(uint64_t scan_rows, b2_batch* out) {
-    cols.clear();
-    uint64_t budget = std::max<uint64_t>(1, std::min<uint64_t>(scan_rows, 1ull << 31));
-    uint64_t produced = 0;
+    const uint64_t budget = begin_scan_batch(scan_rows);
     const bool limited = cp.scan_limit != ~0ull;
-    if (limited && limit_remaining == ~0ull) limit_remaining = cp.scan_limit;
-    if (limited && limit_remaining == 0) drained = true;
-    if (limited && cp.dev.n_conds == 0) budget = std::min<uint64_t>(budget, std::max<uint64_t>(4096, limit_remaining * 2));
+    uint64_t produced = 0;
     if (!desc_started) { desc_started = true; d_unit = units.size(); d_hi = 0; }
     while (!drained && !failed && produced == 0) {
       if (d_hi == 0) {  // next unit down
@@ -1091,10 +1069,7 @@ struct b2_exec {
         }
       }
     }
-    if (limited) {
-      if (produced < limit_remaining) limit_remaining -= produced;
-      else { produced = limit_remaining; limit_remaining = 0; drained = true; }
-    }
+    produced = limit_take(produced);
     if (!failed && !drained && d_hi == 0 && d_unit == 0) drained = true;
     if (!failed && drained && !(limited && limit_remaining == 0)) check_trailing_lock();
     // statistics of the request so far
@@ -1102,18 +1077,12 @@ struct b2_exec {
     tot.last_row = 0;
     fill_stats(tot);
     // reverse the chunk's rows (the kernel wrote them in ascending key order)
-    const size_t n_out = cp.dev.n_out;
     if (produced) {
-      const uint64_t cap = std::max<uint64_t>(64, (produced + 63) & ~63ull);
-      if (cap > rev_cap) {
-        CUDA_TRY(cudaStreamSynchronize(stream));
-        CUDA_TRY(rev_data.reserve(cap * 8 * n_out)); CUDA_TRY(rev_bitmap.reserve(cap / 8 * n_out));
-        rev_cap = cap;
-      }
-      CUDA_TRY(cudaMemsetAsync(rev_bitmap.p, 0xff, rev_cap / 8 * n_out, stream));
+      int rc = reserve_out(&rev_data, &rev_bitmap, &rev_cap, produced);
+      if (rc) return rc;
       // (a Limit may have cut the chunk: the first `produced` rows of the reversed order are the last ones the kernel wrote)
       CUDA_TRY(launch_reverse_rows((const unsigned long long*)out_data.p, (const unsigned long long*)out_bitmap.p, out_cap, (unsigned long long*)rev_data.p,
-                                   (unsigned long long*)rev_bitmap.p, rev_cap, chunk_total, produced, (uint32_t)n_out, stream));
+                                   (unsigned long long*)rev_bitmap.p, rev_cap, chunk_total, produced, (uint32_t)cp.dev.n_out, stream));
       stats.kernel_launches++;
     }
     return publish_scan_columns(produced, out, &rev_data, &rev_bitmap, rev_cap);
@@ -1182,10 +1151,6 @@ struct b2_exec {
   Counters good_ctr{};       // device counters after the last batch that completed without an error
   DevBuf range_rows_prev;
   uint64_t limit_remaining = ~0ull;
-  int scan_grid = 0;
-  DevBuf trace_buf;
-  bool trace_done = false;
-  size_t scan_smem = ~(size_t)0;
 
   void lock_failure(uint32_t r) {
     fail(range_lock_err[r], "key is locked, lock_version=" + std::to_string(range_lock_ts[r]));
@@ -1197,40 +1162,49 @@ struct b2_exec {
       if (range_lock_err[r]) { lock_failure((uint32_t)r); return; }
   }
 
+  // Fixed-width output columns (scan, aggregation and TopN results), one per output offset: fills `cols` and `last_dev`.
+  // Host output copies each column's `n_rows` cells of `esz` bytes and `bm_bytes` of its bitmap into pinned memory.
+  struct FixedCol { const void* data; const void* bitmap; size_t esz, bm_bytes; };
+  int publish_fixed(const std::vector<FixedCol>& fc, uint64_t n_rows) {
+    const bool to_host = out_loc == B2_LOC_HOST && n_rows;
+    cols.assign(fc.size(), b2_column{});
+    last_dev.assign(fc.size(), DevColRef{});
+    last_rows = n_rows;
+    if (to_host) {
+      size_t total = 0;
+      for (const FixedCol& f : fc) total += n_rows * f.esz + f.bm_bytes;
+      CUDA_TRY(h_out.reserve(total));
+    }
+    uint8_t* hp = (uint8_t*)h_out.p;
+    for (size_t i = 0; i < fc.size(); ++i) {
+      const FixedCol& f = fc[i];
+      const OutCol& oc = cp.schema[cp.output_offsets[i]];
+      cols[i].kind = oc.kind; cols[i].field_tp = oc.field_tp; cols[i].field_flag = oc.field_flag; cols[i].len = n_rows;
+      last_dev[i] = DevColRef{f.data, (const unsigned long long*)f.bitmap, oc.kind, oc.field_tp, oc.field_flag};
+      if (to_host) {
+        const size_t bytes = n_rows * f.esz;
+        CUDA_TRY(cudaMemcpyAsync(hp, f.data, bytes, cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaMemcpyAsync(hp + bytes, f.bitmap, f.bm_bytes, cudaMemcpyDeviceToHost, stream));
+        cols[i].data = hp; cols[i].null_bitmap = (const uint64_t*)(hp + bytes);
+        hp += bytes + f.bm_bytes;
+        d2h_bytes += bytes + f.bm_bytes;
+      } else if (n_rows) {
+        cols[i].data = f.data; cols[i].null_bitmap = (const uint64_t*)f.bitmap;
+      }
+    }
+    if (to_host) CUDA_TRY(cudaStreamSynchronize(stream));
+    return B2_OK;
+  }
+
   int publish_scan_columns(uint64_t n_rows, b2_batch* out, const DevBuf* src_data = nullptr, const DevBuf* src_bitmap = nullptr, uint64_t src_cap = 0) {
-    size_t n_out = cp.dev.n_out;
-    cols.resize(n_out);
+    const size_t n_out = cp.dev.n_out;
     const uint8_t* data = (const uint8_t*)(src_data ? src_data->p : out_data.p);
     const uint8_t* bm = (const uint8_t*)(src_bitmap ? src_bitmap->p : out_bitmap.p);
     const uint64_t out_cap = src_data ? src_cap : this->out_cap;
-    if (out_loc == B2_LOC_HOST && n_rows) {
-      size_t per_col = n_rows * 8, per_bm = ((n_rows + 63) / 64) * 8;
-      CUDA_TRY(h_out.reserve((per_col + per_bm) * n_out));
-      uint8_t* hp = (uint8_t*)h_out.p;
-      for (size_t k = 0; k < n_out; ++k) {
-        CUDA_TRY(cudaMemcpyAsync(hp + k * per_col, data + k * out_cap * 8, per_col, cudaMemcpyDeviceToHost, stream));
-        CUDA_TRY(cudaMemcpyAsync(hp + n_out * per_col + k * per_bm, bm + k * (out_cap / 8), per_bm, cudaMemcpyDeviceToHost, stream));
-      }
-      CUDA_TRY(cudaStreamSynchronize(stream));
-      d2h_bytes += (per_col + per_bm) * n_out;
-      for (size_t k = 0; k < n_out; ++k) {
-        cols[k].data = hp + k * per_col;
-        cols[k].null_bitmap = (const uint64_t*)(hp + n_out * per_col + k * per_bm);
-      }
-    } else {
-      for (size_t k = 0; k < n_out; ++k) {
-        cols[k].data = n_rows ? data + k * out_cap * 8 : nullptr;
-        cols[k].null_bitmap = n_rows ? (const uint64_t*)(bm + k * (out_cap / 8)) : nullptr;
-      }
-    }
-    last_dev.assign(n_out, DevColRef{});
-    last_rows = n_rows;
-    for (size_t k = 0; k < n_out; ++k) {
-      const OutCol& oc = cp.schema[cp.dev.mode == PM_SCAN ? cp.output_offsets[k] : k];
-      cols[k].kind = oc.kind; cols[k].field_tp = oc.field_tp; cols[k].field_flag = oc.field_flag; cols[k].len = n_rows;
-      cols[k].offsets = nullptr;
-      last_dev[k] = DevColRef{data + k * out_cap * 8, (const unsigned long long*)(bm + k * (out_cap / 8)), oc.kind, oc.field_tp, oc.field_flag};
-    }
+    std::vector<FixedCol> fc(n_out);
+    for (size_t k = 0; k < n_out; ++k) fc[k] = FixedCol{data + k * out_cap * 8, bm + k * (out_cap / 8), 8, ((n_rows + 63) / 64) * 8};
+    int rc = publish_fixed(fc, n_rows);
+    if (rc) return rc;
     // bytes / json / decimal columns: the 8-byte cells above are references; the column itself is the heap the raw_* kernels filled
     if (cp.dev.n_raw && n_rows) {
       size_t need = 0;
@@ -1469,9 +1443,8 @@ struct b2_exec {
     if (P.has_group && P.n_group <= 1) {
       // direct-addressed: accumulators of the group keys 0 .. slots-1 (+ 4 bytes of occupancy each); 1024 slots of COUNT + SUM
       // are 28 KB, which still lets three CTAs share an SM
-      static const uint32_t want = [] { const char* v = getenv("B2_AGG_DIRECT_SLOTS"); return v ? (uint32_t)atoi(v) : 1024u; }();
-      fast_slots = want;
-      while (fast_slots > 64 && (size_t)fast_slots * (4 + 8 * P.acc_words) > 28 * 1024 * (want / 1024 ? want / 1024 : 1)) fast_slots >>= 1;
+      fast_slots = 1024;
+      while (fast_slots > 64 && (size_t)fast_slots * (4 + 8 * P.acc_words) > 28 * 1024) fast_slots >>= 1;
       fast_smem = ((size_t)fast_slots * (4 + 8 * P.acc_words) + 15) & ~(size_t)15;
     }
     Counters c;
@@ -1562,34 +1535,14 @@ struct b2_exec {
       CUDA_TRY(launch_agg_result(P, n_groups, gk, gn, ga, (unsigned long long**)res_ptrs.p, (unsigned long long**)res_ptrs.p + ncol, stream));
     }
     // deliver the requested output offsets
-    size_t n_out = cp.output_offsets.size();
-    cols.assign(n_out, b2_column{});
-    last_dev.assign(n_out, DevColRef{});
-    last_rows = n_groups;
-    size_t host_off = 0;
-    if (out_loc == B2_LOC_HOST && n_groups) {
-      size_t total = 0;
-      for (size_t i = 0; i < n_out; ++i) total += (size_t)n_groups * (cp.schema[cp.output_offsets[i]].kind == B2_COL_DECIMAL ? 40 : 8) + bm_bytes;
-      CUDA_TRY(h_out.reserve(total));
-    }
+    const size_t n_out = cp.output_offsets.size();
+    std::vector<FixedCol> fc(n_out);
     for (size_t i = 0; i < n_out; ++i) {
-      uint32_t k = cp.output_offsets[i];
-      const OutCol& oc = cp.schema[k];
-      size_t esz = oc.kind == B2_COL_DECIMAL ? 40 : 8;
-      cols[i].kind = oc.kind; cols[i].field_tp = oc.field_tp; cols[i].field_flag = oc.field_flag; cols[i].len = n_groups;
-      last_dev[i] = DevColRef{res_cols[k].p, (const unsigned long long*)res_bitmaps[k].p, oc.kind, oc.field_tp, oc.field_flag};
-      if (out_loc == B2_LOC_HOST && n_groups) {
-        uint8_t* hp = (uint8_t*)h_out.p + host_off;
-        CUDA_TRY(cudaMemcpyAsync(hp, res_cols[k].p, (size_t)n_groups * esz, cudaMemcpyDeviceToHost, stream));
-        CUDA_TRY(cudaMemcpyAsync(hp + (size_t)n_groups * esz, res_bitmaps[k].p, bm_bytes, cudaMemcpyDeviceToHost, stream));
-        cols[i].data = hp; cols[i].null_bitmap = (const uint64_t*)(hp + (size_t)n_groups * esz);
-        host_off += (size_t)n_groups * esz + bm_bytes;
-        d2h_bytes += (size_t)n_groups * esz + bm_bytes;
-      } else {
-        cols[i].data = n_groups ? res_cols[k].p : nullptr;
-        cols[i].null_bitmap = n_groups ? (const uint64_t*)res_bitmaps[k].p : nullptr;
-      }
+      const uint32_t k = cp.output_offsets[i];
+      fc[i] = FixedCol{res_cols[k].p, res_bitmaps[k].p, (size_t)(cp.schema[k].kind == B2_COL_DECIMAL ? 40 : 8), bm_bytes};
     }
+    int rc = publish_fixed(fc, n_groups);
+    if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(stream));
     out->columns = cols.data(); out->n_columns = (uint32_t)n_out; out->n_rows = n_groups; out->n_warnings = 0;
     out->is_drained = B2_DRAIN_DRAINED;
@@ -1678,11 +1631,11 @@ struct b2_exec {
             TopNLists nxt;
             nxt.n_lists = (cur.n_lists + 15) / 16; nxt.stride = limit;
             nxt.items = (TopItem*)(flip ? tn_lvl_b.p : tn_lvl_a.p); nxt.counts = (unsigned int*)(flip ? tn_lvl_b_cnt.p : tn_lvl_a_cnt.p);
-            CUDA_TRY(launch_topn_merge(P, cur, nxt, cap, 16, stream));
+            CUDA_TRY(launch_topn_merge(P, cur, nxt, 16, stream));
             stats.kernel_launches++;
             cur = nxt; flip ^= 1;
           }
-          CUDA_TRY(launch_topn_merge(P, cur, unit_out, cap, cur.n_lists, stream));
+          CUDA_TRY(launch_topn_merge(P, cur, unit_out, cur.n_lists, stream));
         }
         CUDA_TRY(launch_topn_gather(P, a, unit_items, unit_cnt, (unsigned long long*)tn_blk_pay.p, (unsigned char*)tn_blk_null.p, limit, stream));
         // running top-N + the chunk's top-N -> the other buffer set, which becomes the running one
@@ -1717,27 +1670,15 @@ struct b2_exec {
       CUDA_TRY(tn_bitmap.reserve((size_t)n_out * words * 8));
       CUDA_TRY(launch_pack_nulls((const unsigned char*)tn_run_null.p, n_out, limit, n, (unsigned long long*)tn_bitmap.p, words, stream));
     }
-    size_t n_sel = cp.output_offsets.size();
-    cols.assign(n_sel, b2_column{});
-    last_dev.assign(n_sel, DevColRef{});
-    last_rows = n;
-    if (out_loc == B2_LOC_HOST && n) CUDA_TRY(h_out.reserve(n_sel * ((size_t)n * 8 + (size_t)words * 8)));
-    for (size_t i = 0; i < n_sel; ++i) {
-      uint32_t k = cp.output_offsets[i];
-      const OutCol& oc = cp.schema[k];
-      cols[i].kind = oc.kind; cols[i].field_tp = oc.field_tp; cols[i].field_flag = oc.field_flag; cols[i].len = n;
-      if (!n) continue;
-      const uint8_t* d = (const uint8_t*)tn_run_pay.p + (size_t)k * limit * 8;
-      const uint8_t* bm = (const uint8_t*)tn_bitmap.p + (size_t)k * words * 8;
-      last_dev[i] = DevColRef{d, (const unsigned long long*)bm, oc.kind, oc.field_tp, oc.field_flag};
-      if (out_loc == B2_LOC_HOST) {
-        uint8_t* hp = (uint8_t*)h_out.p + i * ((size_t)n * 8 + (size_t)words * 8);
-        CUDA_TRY(cudaMemcpyAsync(hp, d, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
-        CUDA_TRY(cudaMemcpyAsync(hp + (size_t)n * 8, bm, (size_t)words * 8, cudaMemcpyDeviceToHost, stream));
-        cols[i].data = hp; cols[i].null_bitmap = (const uint64_t*)(hp + (size_t)n * 8);
-        d2h_bytes += (size_t)n * 8 + (size_t)words * 8;
-      } else { cols[i].data = d; cols[i].null_bitmap = (const uint64_t*)bm; }
+    const size_t n_sel = cp.output_offsets.size();
+    std::vector<FixedCol> fc(n_sel, FixedCol{nullptr, nullptr, 8, (size_t)words * 8});
+    for (size_t i = 0; i < n_sel && n; ++i) {
+      const uint32_t k = cp.output_offsets[i];
+      fc[i].data = (const uint8_t*)tn_run_pay.p + (size_t)k * limit * 8;
+      fc[i].bitmap = (const uint8_t*)tn_bitmap.p + (size_t)k * words * 8;
     }
+    rc = publish_fixed(fc, n);
+    if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(stream));
     out->columns = cols.data(); out->n_columns = (uint32_t)n_sel; out->n_rows = n; out->n_warnings = 0;
     out->is_drained = B2_DRAIN_DRAINED;
@@ -1809,9 +1750,7 @@ int32_t b2_exec_open(const b2_dag_plan* plan, const b2_key_range* ranges, uint32
   h->device = src->device;
   cudaError_t e = cudaSetDevice(h->device);
   if (e != cudaSuccess) { g_last_error = std::string("cudaSetDevice: ") + cudaGetErrorString(e) + " (the CUDA device path is required; there is no CPU fallback)"; return B2_ERR_CUDA; }
-  if (cfg && cfg->cuda_stream) { h->stream = (cudaStream_t)cfg->cuda_stream; h->own_stream = false; }
-  else { e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking); if (e != cudaSuccess) { g_last_error = cudaGetErrorString(e); return B2_ERR_CUDA; } h->own_stream = true; }
-  e = cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking);
+  e = h->open_streams(cfg);
   if (e != cudaSuccess) { g_last_error = cudaGetErrorString(e); return B2_ERR_CUDA; }
   h->out_loc = cfg ? cfg->output_location : B2_LOC_DEVICE;
   h->deadline_ns = cfg ? cfg->deadline_ns : 0;
@@ -1837,16 +1776,16 @@ int32_t b2_exec_open(const b2_dag_plan* plan, const b2_key_range* ranges, uint32
   if (h->cp.dev.fast_v1 && !h->sample_is_v1()) h->cp.dev.fast_v1 = 0;
   // plan-specialised kernel: B2_JIT=off|sync|auto (environment) overrides cfg->jit; `auto` compiles in the background
   // for requests big enough to matter and switches over when the kernel is ready
-  h->jit_mode = cfg ? cfg->jit : b2_exec::JIT_AUTO;
-  if (const char* ev = getenv("B2_JIT")) h->jit_mode = !strcmp(ev, "off") ? b2_exec::JIT_OFF : (!strcmp(ev, "sync") ? b2_exec::JIT_SYNC : b2_exec::JIT_AUTO);
+  h->jit_mode = cfg ? cfg->jit : B2_JIT_AUTO;
+  if (const char* ev = getenv("B2_JIT")) h->jit_mode = !strcmp(ev, "off") ? B2_JIT_OFF : (!strcmp(ev, "sync") ? B2_JIT_SYNC : B2_JIT_AUTO);
   if (plan_uses_ext_sigs(h->cp.dev)) {  // DIV / MOD / IF / CASE ...: only compiled into specialised kernels (b2_device.h)
     if (!jit_available()) { g_last_error = "this plan's scalar functions need the run-time compiler (libnvrtc), which is not available"; return B2_ERR_UNSUPPORTED; }
-    h->jit_mode = b2_exec::JIT_SYNC;
+    h->jit_mode = B2_JIT_SYNC;
   }
   uint64_t total_entries = 0;
   for (const Unit& u : h->units) total_entries += u.e_hi - u.e_lo;
-  if (h->jit_mode == b2_exec::JIT_SYNC || (h->jit_mode == b2_exec::JIT_AUTO && total_entries >= (1u << 20))) h->jit_start();
-  if (h->jit_mode == b2_exec::JIT_SYNC && h->jit_started) {
+  if (h->jit_mode == B2_JIT_SYNC || (h->jit_mode == B2_JIT_AUTO && total_entries >= (1u << 20))) h->jit_start();
+  if (h->jit_mode == B2_JIT_SYNC && h->jit_started) {
     const JitKernel* k = h->jit_fut.get();
     if (!k->ok) { g_last_error = "plan-specialised kernel: " + k->error; return B2_ERR_CUDA; }
   }
@@ -2055,7 +1994,7 @@ int32_t b2_region_pin(int32_t device, uint64_t region_id, uint64_t data_version,
     if (src->dflt) copy_blocks(src->dflt, src->n_dflt, &pr->dflt);
     if (ok && cudaStreamSynchronize(st) != cudaSuccess) ok = false;
     cudaStreamDestroy(st);
-    if (!ok) { for (auto& b : pr->bufs) b.release(); g_last_error = "block cache: device allocation or copy failed"; return B2_ERR_CUDA; }
+    if (!ok) { g_last_error = "block cache: device allocation or copy failed"; return B2_ERR_CUDA; }
     if (src->lock && src->lock->n) {  // keep a private host copy of CF_LOCK
       const b2_cf_block& L = *src->lock;
       pr->lock_host.resize(2);
@@ -2084,7 +2023,6 @@ int32_t b2_region_unpin(int32_t device, uint64_t region_id, uint64_t data_versio
   if (--it->second->refs > 0) return B2_OK;
   cudaSetDevice(device);
   cudaDeviceSynchronize();  // requests still reading the cached blocks
-  for (auto& b : it->second->bufs) b.release();
   g_cache_bytes[device] -= it->second->bytes;
   region_cache().erase(it);
   return B2_OK;
@@ -2104,9 +2042,7 @@ int32_t b2_checksum_handle(const b2_key_range* ranges, uint32_t n_ranges, const 
   h->device = src->device;
   cudaError_t e = cudaSetDevice(h->device);
   if (e != cudaSuccess) { g_last_error = std::string("cudaSetDevice: ") + cudaGetErrorString(e); return B2_ERR_CUDA; }
-  if (cfg && cfg->cuda_stream) h->stream = (cudaStream_t)cfg->cuda_stream;
-  else { if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return B2_ERR_CUDA; h->own_stream = true; }
-  if (cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking) != cudaSuccess) return B2_ERR_CUDA;
+  if (h->open_streams(cfg) != cudaSuccess) return B2_ERR_CUDA;
   memset(&h->cp.dev, 0, sizeof(h->cp.dev));
   h->cp.dev.mode = PM_CHECKSUM;
   int rc = h->setup_source(src, ranges, n_ranges);
@@ -2116,18 +2052,13 @@ int32_t b2_checksum_handle(const b2_key_range* ranges, uint32_t n_ranges, const 
   // crc register after the old prefix (checksum.rs:75-76 prefix_digest)
   uint64_t st = ~0ull;
   for (uint32_t i = 0; i < old_prefix_len; ++i) st = crc64_table_entry((uint8_t)(st ^ old_prefix[i])) ^ (st >> 8);
-  DevBuf d_prefix;
-  if (d_prefix.reserve(new_prefix_len + 16) != cudaSuccess) return B2_ERR_CUDA;
-  if (new_prefix_len) cudaMemcpyAsync(d_prefix.p, new_prefix, new_prefix_len, cudaMemcpyHostToDevice, h->stream);
-  if (new_prefix_len > 32) { g_last_error = "new_prefix longer than 32 bytes"; d_prefix.release(); return B2_ERR_UNSUPPORTED; }
-  size_t ck_smem = ~(size_t)0;
-  int ck_grid = 0;
+  if (new_prefix_len > 32) { g_last_error = "new_prefix longer than 32 bytes"; return B2_ERR_UNSUPPORTED; }
   h->cp.dev.read_ts = h->read_ts; h->cp.dev.isolation = h->isolation;
   for (size_t ui = 0; ui < h->units.size(); ++ui) {
     const Unit& u = h->units[ui];
     BlockView v;
     rc = h->acquire_block(u.block_idx, &v);
-    if (rc) { d_prefix.release(); return rc; }
+    if (rc) return rc;
     ScanArgs a = h->base_args(u, v);
     a.c_lo = u.e_lo; a.c_hi = u.e_hi;
     a.ck_init_state = st; a.ck_new_prefix_len = new_prefix_len; a.ck_old_prefix_len = old_prefix_len;
@@ -2146,16 +2077,14 @@ int32_t b2_checksum_handle(const b2_key_range* ranges, uint32_t n_ranges, const 
       for (uint32_t j = new_prefix_len; j < 11; ++j) ks = crc64_table_entry((uint8_t)(ks ^ raw[j])) ^ (ks >> 8);
       a.ck_key_state = ks;
     }
-    (void)ck_smem; (void)ck_grid;
     rc = h->launch_unit(a, u, fast, scan_crc_table_bytes(), fast_checksum_bytes(), 0, nullptr, nullptr);
-    if (rc) { d_prefix.release(); return rc; }
+    if (rc) return rc;
     h->release_block(u.block_idx);
     h->prefetch_after(ui);
     h->entries_scanned += u.e_hi - u.e_lo;
   }
   Counters c;
   rc = h->read_counters(&c);
-  d_prefix.release();
   if (rc) return rc;
   h->fill_stats(c);
   if (stats) *stats = h->stats;
@@ -2185,8 +2114,6 @@ int32_t b2_gen_create(int32_t device, const b2_gen_spec* spec, b2_gen** out, b2_
   if (cudaSetDevice(device) != cudaSuccess) { g_last_error = "cudaSetDevice failed"; return B2_ERR_CUDA; }
   std::unique_ptr<b2_gen> g(new b2_gen());
   g->device = device;
-  auto fail = [&](int st, const std::string& m) { g_last_error = m; return st; };
-  (void)fail;
   b2_gen_spec s = *spec;
   size_t n = spec->n_rows, nc = spec->n_cols;
 #define GEN_TRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { g_last_error = std::string(#x) + ": " + cudaGetErrorString(_e); return B2_ERR_CUDA; } } while (0)
@@ -2233,8 +2160,7 @@ int32_t b2_gen_create(int32_t device, const b2_gen_spec* spec, b2_gen** out, b2_
 
 void b2_gen_destroy(b2_gen* g) {
   if (!g) return;
-  cudaSetDevice(g->device);
-  for (DevBuf* b : {&g->keys, &g->koff, &g->vals, &g->voff, &g->row_entries, &g->row_vals, &g->scan_tmp, &g->d_lo, &g->d_range, &g->d_null}) b->release();
+  cudaSetDevice(g->device);  // (the buffers go back to this device's pool)
   delete g;
 }
 

@@ -132,13 +132,26 @@ std::mutex g_mu;
 // leaked on purpose: a static destructor would block process exit on compilations still in flight
 std::map<std::string, Entry>& g_cache = *new std::map<std::string, Entry>();
 
+// What a plan-specialised kernel is compiled from: the plan without its launch parameters (ScanArgs carries those) and the
+// variant it needs
+struct JitSpec {
+  std::string literal;
+  int mode;       // scan_body<mode>
+  bool ext_sigs;  // the rarer scalar functions (b2_device.h)
+  int fast;       // bit 0: the lean kernel too, bit 1: table scan (no index-row decoder)
+};
+JitSpec jit_spec(const DevPlan& plan) {
+  DevPlan p = plan;
+  p.read_ts = 0; p.isolation = 0; p.limit = 0;
+  return JitSpec{plan_literal(p), scan_kernel_mode(plan), plan_uses_ext_sigs(plan), (plan_has_fast_kernel(plan) ? 1 : 0) | (plan.idx_cols == 0 ? 2 : 0)};
+}
+
 // ---- on-disk cache of compiled cubins ------------------------------------------------------------------------------
 // One file per (plan shape, kernel instantiation, compiler options, kernel sources): <dir>/<hash>.cubin plus <hash>.key
 // holding the full key (a hash collision or a stale file is detected by comparing it).  Written atomically (rename).
 std::atomic<unsigned long long> g_nvrtc_compiles{0}, g_cache_hits{0};
-std::string cache_key(int mode, bool ext_sigs, int fast /* bit 0: lean kernel too, bit 1: table scan (no index-row decoder) */, const std::string& literal) {
-  const char* defs = getenv("B2_JIT_DEFS");  // experiment switches change the source text
-  return "b2jit5|sm_90a|mode" + std::to_string(mode) + "|ext" + std::to_string((int)ext_sigs) + "|fast" + std::to_string((int)fast) + "|src" + std::to_string(api().src_hash) + "|" + (defs ? defs : "") + "|" + literal;
+std::string cache_key(const JitSpec& j) {
+  return "b2jit5|sm_90a|mode" + std::to_string(j.mode) + "|ext" + std::to_string((int)j.ext_sigs) + "|fast" + std::to_string(j.fast) + "|src" + std::to_string(api().src_hash) + "|" + j.literal;
 }
 std::string cache_path(const std::string& key, const std::string& dir = api().cache_dir) {
   char name[32];
@@ -146,7 +159,6 @@ std::string cache_path(const std::string& key, const std::string& dir = api().ca
   return dir + "/" + name;
 }
 bool cache_load(const std::string& key, std::vector<char>* cubin) {
-  if (getenv("B2_JIT_NO_DISK_CACHE")) return false;
   for (const std::string* dir : {&api().cache_dir, &api().build_cache_dir}) {
     std::string path = cache_path(key, *dir), k, c;
     if (!read_file(path + ".key", &k) || k != key || !read_file(path + ".cubin", &c) || c.empty()) continue;
@@ -156,7 +168,6 @@ bool cache_load(const std::string& key, std::vector<char>* cubin) {
   return false;
 }
 void cache_store(const std::string& key, const std::vector<char>& cubin) {
-  if (getenv("B2_JIT_NO_DISK_CACHE")) return;
   mkdir(api().cache_dir.c_str(), 0755);
   std::string path = cache_path(key), tmp = path + ".tmp" + std::to_string((long)getpid()) + "." + std::to_string((unsigned long long)(uintptr_t)&cubin);
   for (int pass = 0; pass < 2; ++pass) {
@@ -172,25 +183,24 @@ void cache_store(const std::string& key, const std::vector<char>& cubin) {
 }
 
 // NVRTC only (no CUDA context): plan literal -> sm_90a cubin
-bool compile_cubin(int mode, bool ext_sigs, int fast, const std::string& literal, std::vector<char>* cubin, std::string* error) {
+bool compile_cubin(const JitSpec& j, std::vector<char>* cubin, std::string* error) {
   Api& a = api();
-  std::string defs;  // experiment switches: B2_JIT_DEFS="-DX -DY" (part of the cache key through the source text)
-  if (const char* ev = getenv("B2_JIT_DEFS")) { std::string e(ev); size_t i = 0; while ((i = e.find("-D", i)) != std::string::npos) { size_t j = e.find(' ', i); std::string d = e.substr(i + 2, j == std::string::npos ? j : j - i - 2); defs += "#define " + d + " 1\n"; i = j == std::string::npos ? e.size() : j; } }
-  if (fast & 2) defs += "#define B2_NO_IDX 1\n";  // a table scan's kernel carries none of the index-row decoder
+  std::string defs;
+  if (j.fast & 2) defs += "#define B2_NO_IDX 1\n";  // a table scan's kernel carries none of the index-row decoder
   // Plans with the rarer scalar functions (wide projections over DIV / MOD / CASE ...) compile several times faster with the
   // general-path decoders out of line; everything else keeps them inline, on the hot path of the common plans
-  if (ext_sigs) defs += "#define B2_COLD_OUTLINE 1\n";
-  std::string src = defs + "#define B2_NVRTC 1\n#define B2_JIT_PLAN 1\n#include \"fast_kernel.cuh\"\nnamespace b2 { __constant__ const DevPlan kJitPlan =\n" + literal +
+  if (j.ext_sigs) defs += "#define B2_COLD_OUTLINE 1\n";
+  std::string src = defs + "#define B2_NVRTC 1\n#define B2_JIT_PLAN 1\n#include \"fast_kernel.cuh\"\nnamespace b2 { __constant__ const DevPlan kJitPlan =\n" + j.literal +
                     ";\n}\nextern \"C\" __global__ void __launch_bounds__(b2::TILE + 64, 2) b2_scan_jit(const __grid_constant__ b2::ScanArgs A) {\n"
-                    "  b2::scan_body<" + std::to_string(mode) + ">(b2::kJitPlan, A);\n}\n";
-  if (fast & 1)
+                    "  b2::scan_body<" + std::to_string(j.mode) + ">(b2::kJitPlan, A);\n}\n";
+  if (j.fast & 1)
     src += "extern \"C\" __global__ void __launch_bounds__(b2::FK_THREADS, 3) b2_fast_jit(const __grid_constant__ b2::ScanArgs A) {\n"
-           "  b2::fast_body<" + std::to_string(mode) + ">(b2::kJitPlan, A);\n}\n";
+           "  b2::fast_body<" + std::to_string(j.mode) + ">(b2::kJitPlan, A);\n}\n";
   nvrtcProgram prog;
   if (a.CreateProgram(&prog, src.c_str(), "b2_scan_jit.cu", 0, nullptr, nullptr) != NVRTC_SUCCESS) { *error = "nvrtcCreateProgram failed"; return false; }
   std::string inc = "-I" + a.csrc_dir;
   const char* opts[] = {"--gpu-architecture=sm_90a", "--std=c++17", "-lineinfo", "-DB2_NVRTC=1", "-default-device", inc.c_str(), "-I/usr/local/cuda/include",
-                        ext_sigs ? "-DB2_EXT_SIGS=1" : "-DB2_EXT_SIGS=0", "--split-compile=0"};
+                        j.ext_sigs ? "-DB2_EXT_SIGS=1" : "-DB2_EXT_SIGS=0", "--split-compile=0"};
   nvrtcResult rc = a.CompileProgram(prog, (int)(sizeof(opts) / sizeof(opts[0])), opts);
   g_nvrtc_compiles++;
   if (rc != NVRTC_SUCCESS) {
@@ -210,16 +220,16 @@ bool compile_cubin(int mode, bool ext_sigs, int fast, const std::string& literal
   return true;
 }
 
-JitKernel* compile(int device, int mode, bool ext_sigs, int fast, const std::string& literal) {
+JitKernel* compile(int device, const JitSpec& j) {
   Api& a = api();
   JitKernel* k = new JitKernel();
   cudaSetDevice(device);
   cudaFree(nullptr);  // make sure the primary context exists and is current on this thread
-  const std::string key = cache_key(mode, ext_sigs, fast, literal);
+  const std::string key = cache_key(j);
   std::vector<char> cubin;
   if (cache_load(key, &cubin)) g_cache_hits++;
   else {
-    if (!compile_cubin(mode, ext_sigs, fast, literal, &cubin, &k->error)) return k;
+    if (!compile_cubin(j, &cubin, &k->error)) return k;
     cache_store(key, cubin);
   }
   CUmodule mod;
@@ -227,7 +237,7 @@ JitKernel* compile(int device, int mode, bool ext_sigs, int fast, const std::str
   CUfunction fn;
   if (a.ModuleGetFunction(&fn, mod, "b2_scan_jit") != CUDA_SUCCESS) { k->error = "kernel symbol missing"; return k; }
   k->fn = fn;
-  if (fast & 1) {
+  if (j.fast & 1) {
     CUfunction ff;
     if (a.ModuleGetFunction(&ff, mod, "b2_fast_jit") != CUDA_SUCCESS) { k->error = "lean kernel symbol missing"; return k; }
     k->fn_fast = ff;
@@ -258,17 +268,12 @@ static void jit_wait_all_at_exit() {
 std::shared_future<JitKernel*> jit_get(int device, const DevPlan& plan) {
   static std::once_flag at_exit_once;
   std::call_once(at_exit_once, [] { std::atexit(jit_wait_all_at_exit); });
-  DevPlan p = plan;
-  p.read_ts = 0; p.isolation = 0; p.limit = 0;  // launch parameters (ScanArgs), not part of the specialisation
-  std::string key = std::to_string(device) + "|" + plan_literal(p);
+  JitSpec j = jit_spec(plan);
+  std::string key = std::to_string(device) + "|" + j.literal;
   std::lock_guard<std::mutex> lk(g_mu);
   auto it = g_cache.find(key);
   if (it != g_cache.end()) return it->second.fut;
-  std::string literal = key.substr(key.find('|') + 1);
-  const bool ext_sigs = plan_uses_ext_sigs(plan);
-  int mode = plan.mode == PM_SCAN && plan.n_proj ? (int)PM_PROJ : (plan.mode == PM_AGG && plan.n_group > 1 ? (int)PM_AGGM : plan.mode);
-  const int fast = (plan_has_fast_kernel(plan) ? 1 : 0) | (plan.idx_cols == 0 ? 2 : 0);
-  std::shared_future<JitKernel*> fut = std::async(std::launch::async, [device, mode, ext_sigs, fast, literal] { return compile(device, mode, ext_sigs, fast, literal); }).share();
+  std::shared_future<JitKernel*> fut = std::async(std::launch::async, [device, j] { return compile(device, j); }).share();
   g_cache[key].fut = fut;
   return fut;
 }
@@ -282,23 +287,16 @@ bool plan_has_fast_kernel(const DevPlan& plan) {
   return true;
 }
 
-static int jit_mode_of(const DevPlan& plan) { return plan.mode == PM_SCAN && plan.n_proj ? (int)PM_PROJ : (plan.mode == PM_AGG && plan.n_group > 1 ? (int)PM_AGGM : plan.mode); }
-
 // Compile the kernel of `plan` into the on-disk cache without touching a GPU (build machines, ahead-of-time warm-up).
 // 0 = compiled now, 1 = was cached already, negative = failure (message in *error).
 int jit_precompile(const DevPlan& plan, std::string* error) {
   Api& a = api();
   if (!a.rtc_ok) { *error = a.why; return -1; }
-  DevPlan p = plan;
-  p.read_ts = 0; p.isolation = 0; p.limit = 0;
-  const std::string literal = plan_literal(p);
-  const bool ext_sigs = plan_uses_ext_sigs(plan);
-  const int mode = jit_mode_of(plan);
-  const int fast = (plan_has_fast_kernel(plan) ? 1 : 0) | (plan.idx_cols == 0 ? 2 : 0);
-  const std::string key = cache_key(mode, ext_sigs, fast, literal);
+  const JitSpec j = jit_spec(plan);
+  const std::string key = cache_key(j);
   std::vector<char> cubin;
   if (cache_load(key, &cubin)) return 1;
-  if (!compile_cubin(mode, ext_sigs, fast, literal, &cubin, error)) return -1;
+  if (!compile_cubin(j, &cubin, error)) return -1;
   cache_store(key, cubin);
   return 0;
 }

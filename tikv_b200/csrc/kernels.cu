@@ -7,7 +7,7 @@
 //                         flushed into the HBM group table (BatchSimpleAggregation / BatchFastHashAggregation)
 //   scan_kernel<PM_AGGM>  GROUP BY over 2..4 expressions: composite keys in a hash-tagged HBM table
 //                         (BatchSlowHashAggregation; slow_hash_aggr_executor.rs)
-//   scan_kernel<PM_TOPN>  per-CTA candidate buffers + threshold, merged by topn_merge / gathered by topn_gather (BatchTopN)
+//   scan_kernel<PM_TOPN>  per-CTA candidate buffers + threshold, merged by topn_rank_merge / gathered by topn_gather (BatchTopN)
 //   scan_kernel<PM_CHECKSUM>  CRC-64/XZ per KV, XOR-folded (checksum.rs)
 //   agg_finalize / agg_result, topn_*, pack_nulls, bounds: result materialisation; gen_*: synthetic region generator (tooling)
 // The same device body (scan_kernel.cuh) is compiled per plan at run time by jit.cu.
@@ -128,115 +128,9 @@ cudaError_t launch_fast(const DevPlan& plan, const ScanArgs& a, int grid, size_t
 // ---- TopN: merge candidate lists, gather row payloads ------------------------------------------------------------
 size_t topn_smem_bytes(uint32_t cap, int n_order) { return (((size_t)cap * ((size_t)n_order + 2) * 8 + (size_t)cap * 2) + 15) & ~(size_t)15; }
 
-// CTA b streams every item of input lists [b * fan_in, (b + 1) * fan_in) through one threshold buffer and leaves the
-// best `limit`, sorted, in output list b.  The host applies it level by level (fan-in 8) down to a single list.
-__global__ void __launch_bounds__(TILE) topn_merge_kernel(const __grid_constant__ DevPlan P, TopNLists in, TopNLists out, unsigned int cap, unsigned int fan_in,
-                                                         unsigned int rm_bytes /* dynamic shared memory available to the rank merge */) {
-  extern __shared__ __align__(16) unsigned char dyn_smem[];
-  __shared__ unsigned int s_cnt, s_have_thr;
-  __shared__ TopItem s_thr;
-  const TopBuf tb = topbuf_make(dyn_smem, cap, P);
-  const unsigned int tid = threadIdx.x;
-  if (tid == 0) { s_cnt = 0; s_have_thr = 0; }
-  for (unsigned int i = tid; i < cap; i += TILE) tb.idx[i] = (unsigned short)i;
-  __syncthreads();
-  const unsigned int l0 = blockIdx.x * fan_in;
-  const unsigned int l1 = l0 + fan_in < in.n_lists ? l0 + fan_in : in.n_lists;
-  // walk the occupied part of the input lists only: ends[q] = items in lists l0..l0+q
-  unsigned int ends[16];
-  unsigned int total = 0;
-#pragma unroll
-  for (unsigned int q = 0; q < 16; ++q) {
-    if (l0 + q < l1) total += in.counts[l0 + q] < in.stride ? in.counts[l0 + q] : in.stride;
-    ends[q] = total;
-  }
-  // Rank merge: the input lists are sorted and the order is total (ids), so when all their items fit in shared memory
-  // every item finds its output position as own index + the number of smaller items in each other list (binary searches
-  // in shared memory): no sorting network, cost proportional to the items present.
-  const unsigned int rstride = (unsigned int)P.n_order + 2;
-  if ((size_t)total * rstride * 8 <= (size_t)rm_bytes) {
-    unsigned long long* rw = reinterpret_cast<unsigned long long*>(dyn_smem);
-    for (unsigned int f = tid; f < total; f += TILE) {
-      unsigned int q = 0, first = 0;
-#pragma unroll
-      for (unsigned int z = 0; z < 15; ++z)
-        if (f >= ends[z]) { q = z + 1; first = ends[z]; }
-      const TopItem it = in.items[(size_t)(l0 + q) * in.stride + (f - first)];
-      unsigned long long* d = rw + (size_t)f * rstride;
-      for (int k = 0; k < P.n_order; ++k) d[k] = it.w[k];
-      d[P.n_order] = it.id;
-      d[P.n_order + 1] = (unsigned long long)it.nulls | ((unsigned long long)(((l0 + q) << 16) | (f - first)) << 32);
-    }
-    __syncthreads();
-    auto less = [&](const unsigned long long* a, const unsigned long long* b) -> bool {  // item_less on packed words
-      const unsigned int na_all = (unsigned int)a[rstride - 1], nb_all = (unsigned int)b[rstride - 1];
-      for (int k = 0; k < P.n_order; ++k) {
-        const unsigned int na = (na_all >> k) & 1, nb = (nb_all >> k) & 1;
-        int c;
-        if (na || nb) c = (int)nb - (int)na;
-        else c = a[k] < b[k] ? -1 : (a[k] > b[k] ? 1 : 0);
-        if (c == 0) continue;
-        if (P.order[k].desc) c = -c;
-        return c < 0;
-      }
-      return a[P.n_order] < b[P.n_order];
-    };
-    for (unsigned int f = tid; f < total; f += TILE) {
-      unsigned int q = 0, first = 0;
-#pragma unroll
-      for (unsigned int z = 0; z < 15; ++z)
-        if (f >= ends[z]) { q = z + 1; first = ends[z]; }
-      const unsigned long long* me = rw + (size_t)f * rstride;
-      unsigned int rank = f - first;
-      unsigned int lo_z = 0;
-#pragma unroll 1
-      for (unsigned int z = 0; z < 16; ++z) {
-        const unsigned int hi_z = ends[z];
-        if (z != q && hi_z > lo_z) {
-          unsigned int lo = lo_z, hi = hi_z;
-          while (lo < hi) { const unsigned int mid = (lo + hi) >> 1; if (less(rw + (size_t)mid * rstride, me)) lo = mid + 1; else hi = mid; }
-          rank += lo - lo_z;
-        }
-        lo_z = hi_z;
-      }
-      if (rank < (unsigned int)P.limit) {
-        TopItem it;
-        for (int k = 0; k < MAX_ORDER; ++k) it.w[k] = k < P.n_order ? me[k] : 0ull;
-        it.id = me[P.n_order];
-        it.nulls = (unsigned int)me[P.n_order + 1]; it.slot = (unsigned int)(me[P.n_order + 1] >> 32);
-        out.items[(size_t)blockIdx.x * out.stride + rank] = it;
-      }
-    }
-    if (tid == 0) out.counts[blockIdx.x] = total < (unsigned int)P.limit ? total : (unsigned int)P.limit;
-    return;
-  }
-  for (unsigned int base = 0; base < total; base += TILE) {
-    unsigned int f = base + tid;
-    if (f < total) {
-      unsigned int q = 0, first = 0;
-#pragma unroll
-      for (unsigned int z = 0; z < 15; ++z)
-        if (f >= ends[z]) { q = z + 1; first = ends[z]; }
-      const unsigned int l = l0 + q, i = f - first;
-      TopItem it = in.items[(size_t)l * in.stride + i];
-      it.slot = (l << 16) | i;
-      if (!s_have_thr || item_less(it, s_thr, P)) {
-        unsigned int pos = atomicAdd(&s_cnt, 1u);
-        topbuf_put(tb, tb.idx[pos], it);
-      }
-    }
-    __syncthreads();
-    if (s_cnt + TILE > cap) cta_topn_compact(tb, (unsigned int)P.limit, &s_cnt, &s_have_thr, &s_thr, P);
-  }
-  __syncthreads();
-  cta_topn_compact(tb, (unsigned int)P.limit, &s_cnt, &s_have_thr, &s_thr, P);
-  unsigned int keep = s_cnt;
-  for (unsigned int i = tid; i < keep; i += TILE) out.items[(size_t)blockIdx.x * out.stride + i] = topbuf_get(tb, tb.idx[i]);
-  if (tid == 0) out.counts[blockIdx.x] = keep;
-}
-
-// The same merge without a shared-memory budget: the input lists are sorted and the order is total (ids), so an item's
-// output position is its own index + the number of items that come before it in each sibling list.  Every item is
+// The CTAs of blockIdx.x = b merge input lists [b * fan_in, (b + 1) * fan_in) into output list b: the best `limit` items,
+// sorted.  The host applies it level by level (fan-in 16) down to a single list.  The input lists are sorted and the order
+// is total (ids), so an item's output position is its own index + the number of items that come before it in each sibling list.  Every item is
 // independent: blockIdx.y splits a group's items over as many CTAs as the occupied part needs, and a thread runs its
 // (up to 15) binary searches in lockstep so that their L2 round trips overlap.  Only the first `limit - i` items of a
 // sibling can keep item i inside the output, which bounds every search.  Cost follows the items present.
@@ -289,23 +183,14 @@ __global__ void __launch_bounds__(256) topn_rank_merge_kernel(const __grid_const
   }
 }
 
-cudaError_t launch_topn_merge(const DevPlan& plan, const TopNLists& in, const TopNLists& out, uint32_t cap, uint32_t fan_in, cudaStream_t s) {
-  static const bool staged = getenv("B2_TOPN_MERGE_STAGED") != nullptr;  // the shared-memory merge of earlier builds (A/B runs)
-  if (!staged && fan_in <= 16) {
-    const unsigned int groups = (in.n_lists + fan_in - 1) / fan_in;
-    const unsigned int lists = fan_in < in.n_lists ? fan_in : in.n_lists;
-    const unsigned int clip = in.stride < (unsigned int)plan.limit ? in.stride : (unsigned int)plan.limit;
-    unsigned int y = (lists * clip + 255) / 256;
-    if (y < 1) y = 1;
-    if (y > 16) y = 16;  // (a full group then takes four rounds per thread; the usual, nearly empty lists cost the launch of fewer CTAs)
-    topn_rank_merge_kernel<<<dim3(groups, y), 256, 0, s>>>(plan, in, out, fan_in);
-    return cudaGetLastError();
-  }
-  size_t smem = std::max<size_t>(topn_smem_bytes(cap, plan.n_order), 200 * 1024);  // room for the rank merge: 6400 items of two sort keys
-  static size_t attr_bytes = 0;  // (one process drives one device)
-  if (smem > attr_bytes) { cudaFuncSetAttribute(topn_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr_bytes = smem; }
-  unsigned int grid = (in.n_lists + fan_in - 1) / fan_in;
-  topn_merge_kernel<<<grid, TILE, smem, s>>>(plan, in, out, cap, fan_in, (unsigned int)smem);
+cudaError_t launch_topn_merge(const DevPlan& plan, const TopNLists& in, const TopNLists& out, uint32_t fan_in, cudaStream_t s) {
+  const unsigned int groups = (in.n_lists + fan_in - 1) / fan_in;
+  const unsigned int lists = fan_in < in.n_lists ? fan_in : in.n_lists;
+  const unsigned int clip = in.stride < (unsigned int)plan.limit ? in.stride : (unsigned int)plan.limit;
+  unsigned int y = (lists * clip + 255) / 256;
+  if (y < 1) y = 1;
+  if (y > 16) y = 16;  // (a full group then takes four rounds per thread; the usual, nearly empty lists cost the launch of fewer CTAs)
+  topn_rank_merge_kernel<<<dim3(groups, y), 256, 0, s>>>(plan, in, out, fan_in);
   return cudaGetLastError();
 }
 

@@ -72,8 +72,6 @@ struct ScanArgs {
   uint64_t out_cap;
   // PM_AGG
   AggTable tbl;
-  uint32_t smem_slots;              // per-CTA table slots (power of two), 0 = disabled
-  unsigned long long* trace;        // debug (B2_TRACE=1): per-tile clock64 stamps of CTA 0, 8 words per tile
   uint32_t staging;                 // 1: stage tiles through shared memory with bulk copies
   uint32_t stage_off;               // byte offset of the stages inside dynamic shared memory (multiple of 16)
   uint32_t out_stage_off;           // PM_SCAN: byte offset of the output transpose buffer (multiple of 16)
@@ -84,7 +82,8 @@ struct ScanArgs {
   unsigned int* slow_list;          // capacity >= c_hi - c_lo
   unsigned int* slow_count;
   uint32_t list_mode;               // scan_body: 1 = process the entries of slow_list (count read on the device) instead of [c_lo, c_hi)
-  uint32_t _pad2;
+  uint32_t smem_slots;              // PM_AGG: per-CTA table slots (power of two), 0 = disabled.  Kept in this padding slot: every
+                                    //    other field keeps its alignment, which decides how the kernels load their parameters
   uint64_t ck_key_state;            // lean checksum: crc register after old_prefix and the unit's common raw key bytes [new_prefix_len, 11)
   uint32_t desc;                    // backward scan (TableScan.desc): TopN ties go to the larger key (item ids are complemented)
   uint32_t _pad3;
@@ -131,8 +130,9 @@ cudaError_t launch_agg_finalize(const DevPlan& plan, const AggTable& t, Counters
                                 unsigned long long* out_acc, cudaStream_t s);
 cudaError_t launch_agg_result(const DevPlan& plan, unsigned int n_groups, const unsigned long long* g_keys, const unsigned char* g_null,
                               const unsigned long long* g_acc, unsigned long long** col_data, unsigned long long** col_bitmap, cudaStream_t s);
-// TopN: merge `in` lists into the best `limit` items (sorted) -> out list 0; gather decodes the rows of a list
-cudaError_t launch_topn_merge(const DevPlan& plan, const TopNLists& in, const TopNLists& out, uint32_t cap, uint32_t fan_in, cudaStream_t s);
+// TopN: merge every `fan_in` (<= 16) lists of `in` into the best `limit` items (sorted) -> one list of `out`; gather decodes
+// the rows of a list
+cudaError_t launch_topn_merge(const DevPlan& plan, const TopNLists& in, const TopNLists& out, uint32_t fan_in, cudaStream_t s);
 cudaError_t launch_topn_gather(const DevPlan& plan, const ScanArgs& a, const TopItem* items, const unsigned int* count, unsigned long long* pay,
                                unsigned char* pay_null, uint32_t stride, cudaStream_t s);
 cudaError_t launch_topn_copy(const TopItem* items, const unsigned int* count, uint32_t n_out, uint32_t stride, const unsigned long long* pay0,

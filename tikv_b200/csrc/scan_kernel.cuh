@@ -3,18 +3,6 @@
 #pragma once
 #include "kernels.cuh"
 
-// per-tile clock stamps of CTA 0 (debug builds only: -DB2_TRACE_BUILD; in the product build they cost ~30 instructions per
-// 32 rows for nothing)
-#ifdef B2_TRACE_BUILD
-#define B2_TRACE_STAMP(i) do { if (A.trace && blockIdx.x == 0 && tid == 0 && k < 128) A.trace[k * 8 + (i)] = clock64(); } while (0)
-#define B2_TRACE_T0() long long tc0 = clock64()
-#define B2_TRACE_WAIT() do { if (A.trace && blockIdx.x == 0 && tid == 0 && k < 128) { A.trace[k * 8 + 4] = tc0; A.trace[k * 8 + 5] = clock64(); } } while (0)
-#else
-#define B2_TRACE_STAMP(i) do { } while (0)
-#define B2_TRACE_T0() do { } while (0)
-#define B2_TRACE_WAIT() do { } while (0)
-#endif
-
 namespace b2 {
 
 template <class T> struct b2_remove_cvref { typedef T type; };
@@ -670,12 +658,10 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
     unsigned int warp_off = 0, total = 0, lane_off = 0;
     if (IS_SCAN) {
       // ---- ordered compaction: ballot/popc inside the warp, smem across warps, look-back across tiles ----
-      B2_TRACE_STAMP(0);
       unsigned int bal = __ballot_sync(0xffffffffu, live);
       lane_off = __popc(bal & ((1u << lane) - 1));
       if (lane == 0) s_warp_cnt[k & 1][wid] = __popc(bal);
       cta256_sync();
-      B2_TRACE_STAMP(1);
     } else if (!V::kWholeBlock) {
       cta256_sync();  // the vote below
     }
@@ -704,7 +690,6 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
       // the scan warp may be several tiles behind, other CTAs must not wait for it to get here
       if (tid == 0) atomicExch(&A.tile_status[tile], ((tile == 0 ? 2ull : 1ull) << 62) | total);
       const bool fast = live && row.fast;
-      B2_TRACE_STAMP(2);
       const uint32_t cpc = obuf_cols(total), cshift = cpc == OBUF_COLS ? 2u : 3u, rstride = (OBUF_COLS * TILE) >> cshift;  // columns per chunk (4 or 8), row stride
       const uint32_t n_rounds = P.n_out > 0 ? ((uint32_t)P.n_out + cpc - 1) >> cshift : 1u;
       for (uint32_t r = 0; r < n_rounds; ++r) {
@@ -712,7 +697,6 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
         mbar_wait(&s_obuf_empty[q], ob_phase ^ 1);  // chunk buffer drained (N_OBUF chunks ago)
         if (++ob_q == N_OBUF) { ob_q = 0; ob_phase ^= 1; }
         if (r == 0) {
-          B2_TRACE_STAMP(3);
           // (posted after the wait: at most N_OBUF <= N_CNT - 1 tiles are ever pending at the scan warp)
           if (tid == 0) { s_total[k % N_CNT] = total; s_tile_of[k % N_CNT] = tile; asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&s_cnt_ready[k % N_CNT])) : "memory"); }
         }
@@ -768,7 +752,6 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
         __syncwarp();
         if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&s_obuf_full[q])) : "memory");
       }
-      B2_TRACE_STAMP(7);
     } else if (MODE == PM_TOPN) {
       // BatchTopN: keep the `limit` smallest rows under the order-by key.  A row is a candidate only if it beats
       // the CTA's current threshold (the limit-th best seen so far); candidates are sorted when the buffer fills.
@@ -926,9 +909,7 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
 
   for (uint32_t k = 0;; ++k) {
     const int cur = (int)(k % N_STAGES);
-    B2_TRACE_T0();
     mbar_wait_sleep(&s_full[cur], (k / N_STAGES) & 1);
-    B2_TRACE_WAIT();
     const TileMeta m = s_meta[cur];
     const uint32_t tile = m.tile;
     if (tile >= n_tiles) {
@@ -953,7 +934,6 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
       redo = tile_body(sv, m.w_hi < A.e_hi ? m.w_hi : A.e_hi, k, tile);
     }
     if (redo) tile_body(A.blk, A.e_hi, k, tile);
-    B2_TRACE_STAMP(6);
     __syncwarp();  // this warp is done with stage `cur`: let the producer refill it
     if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&s_empty[cur])) : "memory");
   }

@@ -285,12 +285,21 @@ __global__ void sst_enc_write_kernel(FlatIn F, EncOpt o, const unsigned long lon
   }
 }
 
+// A growable device allocation, freed with the buffer (moving leaves the source empty).  Not pooled on purpose: decoded
+// blocks are large and long-lived.
 struct RawBuf {
   void* p = nullptr;
   size_t cap = 0;
+  RawBuf() = default;
+  RawBuf(RawBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  RawBuf& operator=(RawBuf&& o) noexcept {
+    if (this != &o) { free(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+    return *this;
+  }
+  ~RawBuf() { free(); }
   cudaError_t reserve(size_t n) {
     if (n <= cap) return cudaSuccess;
-    if (p) { cudaFree(p); p = nullptr; cap = 0; }
+    free();
     n = (n + 255) & ~(size_t)255;
     cudaError_t e = cudaMalloc(&p, n);
     if (e == cudaSuccess) cap = n;
@@ -308,10 +317,10 @@ struct b2_sst {
   RawBuf keys, koff, vals, voff;  // decoded block (b2_sst_decode)
   RawBuf enc, enc_offs;           // encoded blocks (b2_sst_encode)
   RawBuf boffs, nres, cnt_n, cnt_k, cnt_v, tmp, err;  // offsets, restart / entry counts and their prefix sums
+  // (the buffers are freed after this, when the handle is deleted: the device is current and the stream drained by then)
   void destroy() {
     cudaSetDevice(device);
     if (stream) cudaStreamSynchronize(stream);
-    for (RawBuf* b : {&enc, &enc_offs, &keys, &koff, &vals, &voff, &boffs, &nres, &cnt_n, &cnt_k, &cnt_v, &tmp, &err}) b->free();
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     if (stream) cudaStreamDestroy(stream);
@@ -327,7 +336,7 @@ struct Staging {
   RawBuf buf;
 };
 Staging* staging_acquire(int device) {
-  static Staging st[64][2];
+  static auto* st = new Staging[64][2];  // leaked on purpose: freeing them at exit would run after the CUDA runtime's teardown
   Staging* a = st[device & 63];
   if (a[0].mu.try_lock()) return &a[0];
   if (a[1].mu.try_lock()) return &a[1];

@@ -6,7 +6,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("B2_LIB") or os.path.join(_HERE, "_build", "libb2copr.so")  # B2_LIB: experimental builds only
+LIB_PATH = os.path.join(_HERE, "_build", "libb2copr.so")
 
 # ---- enums -------------------------------------------------------------------------------------
 B2_OK, B2_ERR_STORAGE, B2_ERR_KEY_IS_LOCKED, B2_ERR_WRITE_CONFLICT, B2_ERR_EVALUATE = 0, 1, 2, 3, 4
