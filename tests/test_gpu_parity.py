@@ -725,6 +725,37 @@ def test_desc_aggregation_topn_errors_and_locks(regions):
     assert exp.status == ffi.B2_ERR_KEY_IS_LOCKED == got.status and got.rows() == exp.rows() and len(got.rows()) == 249
 
 
+@pytest.mark.parametrize("batch", [64, 1 << 22])
+@pytest.mark.parametrize("desc", [False, True], ids=["forward", "backward"])
+def test_scan_error_statistics_match_rows(desc, batch):
+    """A failing row in the middle of a plain scan: the rows the scan meets before it come out, then the error, and the
+    statistics describe exactly those rows (rows per range, processed keys) in both directions, also when the batch
+    that meets the failing row has to be redone."""
+    T = sc.TABLE
+    r = kvfmt.Region()
+    for h in range(500):
+        r.put(kvfmt.row_key(T, h), kvfmt.row_v2([(1, h, "int"), (2, h % 5, "int"), (3, 7, "uint"), (4, 1.0, "f64"), (6, 1, "int")]), 10, 20)
+    r.raw_write(kvfmt.row_key(T, 100), 50, b"Xjunk").raw_write(kvfmt.row_key(T, 400), 50, b"Xjunk")
+    host = r.build(read_ts=100, n_write_blocks=2)
+    ranges = [kvfmt.table_range(T, 0, 300), kvfmt.table_range(T, 300, 500)]
+    plan = Plan().table_scan(T, sc.COLUMNS, desc=desc).build()
+    exp = orc.dag_handle(plan, ranges, host)
+    assert exp.status == ffi.B2_ERR_STORAGE and exp.n_rows == (99 if desc else 100)
+    for region in (host, DeviceRegion(host)):
+        with BatchExecutor(plan, ranges, region) as ex:
+            rows, per_range = [], [0] * len(ranges)
+            while True:
+                b = ex.next_batch(batch)
+                rows += b.rows()
+                for i, n in enumerate(ex.collect_scanned_rows_per_range()):
+                    per_range[i] += n
+                if b.error is not None or b.is_drained:
+                    break
+            assert b.error is not None and b.error.status == exp.status
+            assert rows == exp.rows()
+            assert sum(per_range) == ex.collect_exec_stats().write_processed_keys == len(rows)
+
+
 def test_desc_take_scanned_range(regions):
     """scanner.rs:204-229 with scan_backward_in_range: consecutive takes tile the key space from the top: each lower bound
     is the key of the last (smallest) row returned, the next take's upper bound; the last take reaches the first range's start."""

@@ -271,15 +271,15 @@ struct b2_exec {
   std::vector<std::vector<uint8_t>> range_raw_lo, range_raw_hi;  // the caller's raw bounds (take_scanned_range)
   std::vector<uint8_t> working_begin;                    // RangesScanner::working_range_begin_key (scanner.rs:204-229)
   uint64_t last_row_taken = 0;                           // Counters::last_row at the previous take
-  uint64_t last_row_seen = 0;
+  uint64_t last_row_seen = 0, first_row_seen = ~0ull;    // Counters::last_row / first_row as of the last batch
   DevBuf range_rows;                                     // per range: rows returned by the MVCC scan
   std::vector<uint64_t> range_rows_taken;                // already handed out by collect_scanned_rows_per_range
   std::vector<int> range_lock_err;                      // 1 = range ends with KeyIsLocked
   std::vector<uint64_t> range_lock_ts;
   std::vector<Unit> units;
   uint32_t first_live_range = 0;                         // backward scans: ranges below a conflicting lock's range are never reached
-  size_t cur_unit = 0;
-  uint32_t cur_entry = 0;
+  size_t cur_unit = 0;                                   // PM_SCAN cursor: the unit being consumed and what is left of it
+  uint32_t cur_lo = 0, cur_hi = 0;
   bool started = false, drained = false, failed = false;
   bool saw_lock = false;
   uint64_t lock_keys_seen = 0;
@@ -658,10 +658,9 @@ struct b2_exec {
   int init_device_state() {
     CUDA_TRY(ctr_buf.reserve(sizeof(Counters)));
     CUDA_TRY(h_ctr.reserve(sizeof(Counters)));
-    Counters z;
-    memset(&z, 0, sizeof(z));
-    z.err = ~0ull; z.first_row = ~0ull;
-    CUDA_TRY(cudaMemcpyAsync(ctr_buf.p, &z, sizeof(z), cudaMemcpyHostToDevice, stream));
+    memset(&good_ctr, 0, sizeof(good_ctr));
+    good_ctr.err = ~0ull; good_ctr.first_row = ~0ull;
+    CUDA_TRY(cudaMemcpyAsync(ctr_buf.p, &good_ctr, sizeof(good_ctr), cudaMemcpyHostToDevice, stream));
     CUDA_TRY(range_rows.reserve(std::max<size_t>(1, range_raw_lo.size()) * 8));
     CUDA_TRY(cudaMemsetAsync(range_rows.p, 0, std::max<size_t>(1, range_raw_lo.size()) * 8, stream));
     range_rows_taken.assign(range_raw_lo.size(), 0);
@@ -694,7 +693,7 @@ struct b2_exec {
     kev_used = 0;
   }
   void fill_stats(const Counters& c) {
-    last_row_seen = c.last_row;
+    last_row_seen = c.last_row; first_row_seen = c.first_row;
     stats.write_entries_scanned = entries_scanned;
     stats.write_processed_keys = c.processed_keys;
     stats.processed_size = c.processed_size;
@@ -703,13 +702,15 @@ struct b2_exec {
     stats.met_newer_ts_data = check_newer ? ((c.met_newer || saw_lock) ? 1 : 0) : -1;
     stats.h2d_bytes = h2d_bytes; stats.d2h_bytes = d2h_bytes;
     met_newer_any = c.met_newer || saw_lock;
-    warnings_total = cp.desc && cp.dev.mode == PM_SCAN ? desc_warnings : c.warn_div0;
+    warnings_total = c.warn_div0;
   }
   bool met_newer_any = false;
 
+  // the failing row a scan in this direction meets first
+  unsigned long long first_error(const Counters& c) const { return cp.desc ? c.err_max : c.err; }
   int device_error(const Counters& c) {
     if (c.err == ~0ull) return B2_OK;
-    const unsigned long long e = cp.desc ? c.err_max : c.err;  // the failing row a scan in this direction meets first
+    const unsigned long long e = first_error(c);
     int status, mysql;
     const char* m = dev_err_message((int)(e & 0xff), &status, &mysql);
     return fail(status, m, mysql, e >> 8);
@@ -816,8 +817,11 @@ struct b2_exec {
   }
 
   // ---- PM_SCAN: up to `scan_rows` CF_WRITE entries per call, appended in key order into one set of columns ----
-  // One pass = one launch per (range, block) unit touched; launches chain on the stream through the device-side
-  // row counter (out_rows -> out_base), so there is a single host sync per batch.
+  // A forward scan consumes the units first to last, each from its lower end.  The rows of a backward scan (TableScan.desc;
+  // scan_executor.rs:89-101, backward.rs:78-225) are the rows of the forward scan in reverse order (the MVCC rule per key
+  // is the same), so it consumes the units last to first, each from its upper end, runs the forward kernel and reverses
+  // the rows on the device.  A launch only emits runs that *start* inside it, and its walks may go past its upper end, so
+  // a version run is never split.
   // output columns (8-byte cells) for `rows` rows in `data` / `bitmap`, their non-NULL bitmaps set to ones
   int reserve_out(DevBuf* data, DevBuf* bitmap, uint64_t* cap_now, uint64_t rows) {
     const size_t n_out = cp.dev.n_out;
@@ -876,219 +880,152 @@ struct b2_exec {
     return produced;
   }
 
-  int run_scan_pass(uint64_t budget, uint64_t stop_before, bool* hit_lock_range, uint32_t* lock_range, Counters* c) {
-    // capacity = entries this pass may cover
-    uint64_t need = 0, left = budget;
-    {
-      size_t u = cur_unit; uint32_t e = cur_entry;
-      while (left && u < units.size()) {
-        uint32_t lo = std::max(e, units[u].e_lo);
-        uint64_t take = std::min<uint64_t>(left, units[u].e_hi - lo);
-        need += take; left -= take;
-        ++u; e = 0;
-      }
+  // the unit a scan consumes after unit `u`; units.size() = none
+  size_t unit_after(size_t u) const { return !cp.desc ? u + 1 : u ? u - 1 : units.size(); }
+  void enter_unit(size_t u) {
+    cur_unit = u;
+    if (u < units.size()) { cur_lo = units[u].e_lo; cur_hi = units[u].e_hi; }
+  }
+  // unit `u` is the last one of its range in scan order (the highest unit of a forward range, the lowest of a backward
+  // one) and that range ends in a conflicting lock
+  bool ends_locked_range(size_t u) const {
+    const size_t next = unit_after(u);
+    return (next >= units.size() || units[next].range_idx != units[u].range_idx) && range_lock_err[units[u].range_idx];
+  }
+
+  // one launch of a pass: the entries [c_lo, c_hi) of unit `unit`; the walks of its last runs stop at `walk_end`
+  struct Piece { size_t unit; uint32_t c_lo, c_hi, walk_end; };
+  // The pieces of the next pass, in ascending key order, taken from the cursor.  `bound` (a global entry index, ~0 = none)
+  // is the failing row an earlier run of this pass met: a forward pass stops before it, a backward pass starts after it.
+  std::vector<Piece> plan_pass(uint64_t budget, uint64_t bound) const {
+    std::vector<Piece> ps;
+    if (cp.desc) {  // one piece of at most `budget` entries from the top of the current unit
+      const Unit& u = units[cur_unit];
+      uint64_t c_lo = (uint64_t)cur_hi - cur_lo > budget ? cur_hi - budget : cur_lo;
+      if (bound != ~0ull) c_lo = std::max<uint64_t>(c_lo, bound - wblocks[u.block_idx].entry_base + 1);
+      if (c_lo < cur_hi) ps.push_back(Piece{cur_unit, (uint32_t)c_lo, cur_hi, u.e_hi});
+      return ps;
     }
-    int rc = reserve_out(&out_data, &out_bitmap, &out_cap, need);
+    // forward: across units up to the budget; a range that ends in a conflicting lock ends the pass
+    for (size_t u = cur_unit; budget && u < units.size(); ++u) {
+      const Unit& U = units[u];
+      const uint64_t base = wblocks[U.block_idx].entry_base;
+      const uint32_t c_lo = u == cur_unit ? cur_lo : U.e_lo;
+      uint32_t c_hi = (uint32_t)std::min<uint64_t>(U.e_hi, (uint64_t)c_lo + budget);
+      const bool cut = bound != ~0ull && base + c_hi > bound;
+      if (cut) c_hi = bound > base + c_lo ? (uint32_t)(bound - base) : c_lo;
+      // (the failing entry is a run start: nothing before it can reach past it)
+      if (c_hi > c_lo) { ps.push_back(Piece{u, c_lo, c_hi, cut ? c_hi : U.e_hi}); budget -= c_hi - c_lo; }
+      if (c_hi < U.e_hi || ends_locked_range(u)) break;
+    }
+    return ps;
+  }
+
+  // One pass: the pieces, each launch appending behind the rows of the launches before it (out_rows -> out_base on the
+  // device), then a single host sync for the counters.  The cursor moves past every piece launched.  *lock_range: the
+  // range whose conflicting lock the pass reached, or -1.
+  int run_scan_pass(uint64_t budget, uint64_t bound, int* lock_range, Counters* c) {
+    const std::vector<Piece> ps = plan_pass(budget, bound);
+    uint64_t rows = 0, vb = 0;
+    int last_blk = -1;
+    for (const Piece& p : ps) {
+      rows += p.c_hi - p.c_lo;
+      const int b = (int)units[p.unit].block_idx;
+      if (b != last_blk) { vb += wblocks[b].val_bytes; last_blk = b; }
+    }
+    int rc = reserve_out(&out_data, &out_bitmap, &out_cap, rows);
     if (rc) return rc;
     if (cp.dev.n_raw) {
       // every byte a cell reference of this pass can point at: the value heaps of the blocks it touches (+ CF_DEFAULT)
-      uint64_t vb = 0;
-      {
-        size_t u = cur_unit; uint64_t l = budget; int last_blk = -1;
-        while (l && u < units.size()) {
-          if ((int)units[u].block_idx != last_blk) { vb += wblocks[units[u].block_idx].val_bytes; last_blk = (int)units[u].block_idx; }
-          uint32_t lo = std::max(u == cur_unit ? cur_entry : 0u, units[u].e_lo);
-          uint64_t take = std::min<uint64_t>(l, units[u].e_hi - lo);
-          l -= take; ++u;
-        }
-        for (const SrcBlock& d : dblocks) vb += d.val_bytes;
-      }
+      for (const SrcBlock& d : dblocks) vb += d.val_bytes;
       CUDA_TRY(cudaStreamSynchronize(stream));
       rc = raw_prepare(out_cap, vb);
       if (rc) return rc;
     }
-    // keep request-level statistics, reset the per-batch row counters
+    // keep request-level statistics, reset the per-pass row counters
     CUDA_TRY(cudaMemsetAsync(&ctr()->out_rows, 0, 8, stream));
     CUDA_TRY(cudaMemsetAsync(&ctr()->out_base, 0, 8, stream));
-    *hit_lock_range = false;
-    while (budget && cur_unit < units.size()) {
-      const Unit& u = units[cur_unit];
+    *lock_range = -1;
+    for (const Piece& p : ps) {
       if (deadline_exceeded()) break;
-      if (cur_entry < u.e_lo) cur_entry = u.e_lo;
-      uint64_t base = wblocks[u.block_idx].entry_base;
-      uint32_t c_lo = cur_entry, c_hi = (uint32_t)std::min<uint64_t>(u.e_hi, (uint64_t)c_lo + budget);
-      bool stop_here = false;
-      if (stop_before != ~0ull && base + c_hi > stop_before) {
-        c_hi = stop_before > base + c_lo ? (uint32_t)(stop_before - base) : c_lo;
-        stop_here = true;
-      }
-      if (c_hi > c_lo) {
-        // (the failing entry is a run start: nothing before it can reach past it)
-        rc = scan_chunk(u, c_lo, c_hi, stop_here ? c_hi : u.e_hi);
-        if (rc) return rc;
-        CUDA_TRY(cudaMemcpyAsync(&ctr()->out_base, &ctr()->out_rows, 8, cudaMemcpyDeviceToDevice, stream));
-        entries_scanned += c_hi - c_lo;
-        budget -= c_hi - c_lo;
-      }
-      cur_entry = c_hi;
-      if (stop_here) break;
-      if (c_hi >= u.e_hi) {
-        prefetch_after(cur_unit);
-        bool range_end = cur_unit + 1 >= units.size() || units[cur_unit + 1].range_idx != u.range_idx;
-        cur_unit++;
-        cur_entry = cur_unit < units.size() ? units[cur_unit].e_lo : 0;
-        if (range_end && range_lock_err[u.range_idx]) { *hit_lock_range = true; *lock_range = u.range_idx; break; }
-      }
+      rc = scan_chunk(units[p.unit], p.c_lo, p.c_hi, p.walk_end);
+      if (rc) return rc;
+      CUDA_TRY(cudaMemcpyAsync(&ctr()->out_base, &ctr()->out_rows, 8, cudaMemcpyDeviceToDevice, stream));
+      entries_scanned += p.c_hi - p.c_lo;
+      if (cp.desc) cur_hi = p.c_lo; else cur_lo = p.c_hi;
+      if (cur_lo < cur_hi) continue;
+      // the unit is done.  prefetch_after stages the blocks of the units after it, which only a forward scan reads next.
+      if (!cp.desc) prefetch_after(p.unit);
+      if (ends_locked_range(p.unit)) *lock_range = (int)units[p.unit].range_idx;
+      enter_unit(unit_after(p.unit));
     }
     return read_counters(c);
   }
 
+  Counters good_ctr{};  // device counters after the last pass that met no failing row (first: what init_device_state uploads)
+  DevBuf range_rows_prev;
+  DevBuf rev_data, rev_bitmap;
+  uint64_t rev_cap = 0;
   int next_scan_batch(uint64_t scan_rows, b2_batch* out) {
     const uint64_t budget = begin_scan_batch(scan_rows);
     const bool limited = cp.scan_limit != ~0ull;
-    uint64_t produced = 0;
-    while (!drained && !failed && produced == 0) {
+    const size_t rr_bytes = std::max<size_t>(1, range_raw_lo.size()) * 8;
+    Counters c = good_ctr;
+    uint64_t written = 0;  // rows the last pass wrote
+    while (!drained && !failed && written == 0) {
       if (cur_unit >= units.size()) { drained = true; break; }
-      size_t save_unit = cur_unit; uint32_t save_entry = cur_entry; uint64_t save_scanned = entries_scanned;
-      // the per-range row counts as they were before this batch (restored if the batch has to be redone)
-      const size_t rr_bytes = std::max<size_t>(1, range_raw_lo.size()) * 8;
+      // what the pass starts from, restored if it meets a failing row
+      const size_t save_unit = cur_unit;
+      const uint32_t save_lo = cur_lo, save_hi = cur_hi;
+      const uint64_t save_scanned = entries_scanned;
       CUDA_TRY(range_rows_prev.reserve_on(stream, rr_bytes));
       CUDA_TRY(cudaMemcpyAsync(range_rows_prev.p, range_rows.p, rr_bytes, cudaMemcpyDeviceToDevice, stream));
-      bool hit_lock = false; uint32_t lock_r = 0;
-      Counters c;
-      int rc = run_scan_pass(budget, ~0ull, &hit_lock, &lock_r, &c);
+      int lock_r;
+      int rc = run_scan_pass(budget, ~0ull, &lock_r, &c);
       if (rc) return rc;
-      fill_stats(c);
-      produced = c.out_rows;
+      written = c.out_rows;
       if (c.err != ~0ull) {
-        // rows before the failing row stay valid (interface.rs:229-235): redo this batch up to it, then report.  The redo
-        // starts from the request-level counters of the batches before this one, so nothing is counted twice and the
-        // statistics describe exactly the rows that were returned (the reference's partial-result semantics).
-        cur_unit = save_unit; cur_entry = save_entry; entries_scanned = save_scanned;
-        Counters z = good_ctr;
-        z.err = ~0ull; z.first_row = ~0ull; z.err_max = 0; z.out_rows = 0; z.out_base = 0;
-        CUDA_TRY(cudaMemcpyAsync(ctr_buf.p, &z, sizeof(z), cudaMemcpyHostToDevice, stream));
+        // the rows the scan meets before the failing row stay valid (interface.rs:229-235): redo the pass up to that row
+        // from the state it started from, so nothing is counted twice and the statistics describe exactly the rows that
+        // were returned (the reference's partial-result semantics)
+        const Counters bad = c;
+        cur_unit = save_unit; cur_lo = save_lo; cur_hi = save_hi; entries_scanned = save_scanned;
+        CUDA_TRY(cudaMemcpyAsync(ctr_buf.p, &good_ctr, sizeof(good_ctr), cudaMemcpyHostToDevice, stream));
         CUDA_TRY(cudaMemcpyAsync(range_rows.p, range_rows_prev.p, rr_bytes, cudaMemcpyDeviceToDevice, stream));
-        Counters c2;
-        rc = run_scan_pass(budget, c.err >> 8, &hit_lock, &lock_r, &c2);
+        rc = run_scan_pass(budget, first_error(bad) >> 8, &lock_r, &c);
         if (rc) return rc;
-        fill_stats(c2);
-        produced = c2.err == ~0ull ? c2.out_rows : 0;
+        written = c.err == ~0ull ? c.out_rows : 0;
         // (the reference never reaches a failing row that lies beyond the rows a Limit still wants)
-        if (!(limited && produced >= limit_remaining)) device_error(c);
+        if (!(limited && written >= limit_remaining)) device_error(bad);
         drained = true;
         break;
       }
       good_ctr = c;
-      if (hit_lock) {
-        if (!(limited && produced >= limit_remaining)) lock_failure(lock_r);
+      if (lock_r >= 0) {
+        if (!(limited && written >= limit_remaining)) lock_failure((uint32_t)lock_r);
         drained = true;
         break;
       }
     }
-    produced = limit_take(produced);
+    fill_stats(c);
+    uint64_t produced = limit_take(written);
     if (!failed && cur_unit >= units.size()) {
       drained = true;
       if (!(limited && limit_remaining == 0)) check_trailing_lock();
     }
     if (cp.dev.n_raw && produced && !raw_outs.empty() && raw_collect() != B2_OK) produced = 0;
-    return publish_scan_columns(produced, out);
-  }
-  // ---- backward scan (TableScan.desc; scan_executor.rs:89-101, backward.rs:78-225) ----
-  // The rows of a backward scan are the rows of the forward scan in reverse order (the MVCC rule per key is the same), so
-  // a batch is one chunk of at most `scan_rows` entries taken from the *end* of what is left — units last to first, inside
-  // a unit from its upper end down — run through the forward kernel and reversed on the device.  A chunk only emits runs
-  // that *start* inside it, and its walks may go past its upper end, so a version run is never split.
-  bool desc_started = false;
-  size_t d_unit = 0;       // unit being consumed (counts down)
-  uint32_t d_hi = 0;       // exclusive upper entry of what is left of it
-  DevBuf rev_data, rev_bitmap;
-  uint64_t rev_cap = 0;
-  int run_desc_chunk(const Unit& u, uint32_t c_lo, uint32_t c_hi, Counters* c) {
-    int rc = reserve_out(&out_data, &out_bitmap, &out_cap, c_hi - c_lo);
-    if (rc) return rc;
-    Counters z;
-    memset(&z, 0, sizeof(z));
-    z.err = ~0ull; z.first_row = ~0ull;
-    // per-chunk counters; request-level statistics are carried on the host (desc_stats)
-    CUDA_TRY(cudaMemcpyAsync(ctr_buf.p, &z, sizeof(z), cudaMemcpyHostToDevice, stream));
-    rc = scan_chunk(u, c_lo, c_hi, u.e_hi);
-    if (rc) return rc;
-    return read_counters(c);
-  }
-  Counters desc_stats{};  // request-level sums of the per-chunk counters
-  uint64_t desc_warnings = 0;
-  void desc_accumulate(const Counters& c) {
-    desc_stats.processed_keys += c.processed_keys; desc_stats.processed_size += c.processed_size; desc_stats.default_lookups += c.default_lookups;
-    desc_stats.met_newer |= c.met_newer; desc_stats.live_rows += c.live_rows; desc_warnings += c.warn_div0;
-    first_row_seen = std::min<uint64_t>(first_row_seen, c.first_row);
-  }
-  int next_scan_batch_desc(uint64_t scan_rows, b2_batch* out) {
-    const uint64_t budget = begin_scan_batch(scan_rows);
-    const bool limited = cp.scan_limit != ~0ull;
-    uint64_t produced = 0;
-    if (!desc_started) { desc_started = true; d_unit = units.size(); d_hi = 0; }
-    while (!drained && !failed && produced == 0) {
-      if (d_hi == 0) {  // next unit down
-        if (d_unit == 0) { drained = true; break; }
-        --d_unit;
-        d_hi = units[d_unit].e_hi;
-      }
-      const Unit& u = units[d_unit];
-      const uint32_t c_hi = d_hi;
-      const uint32_t c_lo = (uint64_t)c_hi - u.e_lo > budget ? (uint32_t)(c_hi - budget) : u.e_lo;
-      Counters c;
-      int rc = run_desc_chunk(u, c_lo, c_hi, &c);
-      if (rc) return rc;
-      entries_scanned += c_hi - c_lo;
-      if (c.err != ~0ull) {
-        // a backward scan meets the failing row with the largest key first: the rows above it stay valid (interface.rs:229-235)
-        const uint64_t base = wblocks[u.block_idx].entry_base;
-        const uint32_t after = (uint32_t)((c.err_max >> 8) - base) + 1;
-        Counters c2;
-        memset(&c2, 0, sizeof(c2));
-        c2.err = ~0ull;
-        if (after < c_hi) { rc = run_desc_chunk(u, after, c_hi, &c2); if (rc) return rc; }
-        produced = c2.err == ~0ull ? c2.out_rows : 0;
-        chunk_total = produced;
-        desc_accumulate(c2);
-        if (!(limited && produced >= limit_remaining)) device_error(c);
-        drained = true;
-        break;
-      }
-      desc_accumulate(c);
-      produced = c.out_rows;
-      chunk_total = produced;
-      d_hi = c_lo > u.e_lo ? c_lo : 0;
-      if (d_hi == 0) {  // the unit is finished; was it the lowest one of a range that ends in a conflicting lock?
-        const bool range_done = d_unit == 0 || units[d_unit - 1].range_idx != u.range_idx;
-        if (range_done && u.range_idx < range_lock_err.size() && range_lock_err[u.range_idx]) {
-          if (!(limited && produced >= limit_remaining)) lock_failure(u.range_idx);
-          drained = true;
-          break;
-        }
-      }
-    }
-    produced = limit_take(produced);
-    if (!failed && !drained && d_hi == 0 && d_unit == 0) drained = true;
-    if (!failed && drained && !(limited && limit_remaining == 0)) check_trailing_lock();
-    // statistics of the request so far
-    Counters tot = desc_stats;
-    tot.last_row = 0;
-    fill_stats(tot);
-    // reverse the chunk's rows (the kernel wrote them in ascending key order)
+    if (!cp.desc) return publish_scan_columns(produced, out);
+    // the kernel wrote the rows in ascending key order.  (A Limit may have cut them: the first `produced` rows of the
+    // reversed order are the last ones the kernel wrote.)
     if (produced) {
       int rc = reserve_out(&rev_data, &rev_bitmap, &rev_cap, produced);
       if (rc) return rc;
-      // (a Limit may have cut the chunk: the first `produced` rows of the reversed order are the last ones the kernel wrote)
       CUDA_TRY(launch_reverse_rows((const unsigned long long*)out_data.p, (const unsigned long long*)out_bitmap.p, out_cap, (unsigned long long*)rev_data.p,
-                                   (unsigned long long*)rev_bitmap.p, rev_cap, chunk_total, produced, (uint32_t)cp.dev.n_out, stream));
+                                   (unsigned long long*)rev_bitmap.p, rev_cap, written, produced, (uint32_t)cp.dev.n_out, stream));
       stats.kernel_launches++;
     }
     return publish_scan_columns(produced, out, &rev_data, &rev_bitmap, rev_cap);
   }
-  uint64_t chunk_total = 0;         // rows the last chunk's kernel wrote
-  uint64_t first_row_seen = ~0ull;  // smallest global entry index a row was returned for so far
 
   // bytes / json / decimal output columns (kernels.cu raw_*): per column an offsets array + byte heap (or decimal structs),
   // a device-resident heap cursor, one error word
@@ -1148,8 +1085,6 @@ struct b2_exec {
     }
     return B2_OK;
   }
-  Counters good_ctr{};       // device counters after the last batch that completed without an error
-  DevBuf range_rows_prev;
   uint64_t limit_remaining = ~0ull;
 
   void lock_failure(uint32_t r) {
@@ -1693,13 +1628,17 @@ struct b2_exec {
     if (deadline_exceeded()) { out->is_drained = B2_DRAIN_DRAINED; return last_err.status; }
     if (!started) {
       started = true;
-      if (cp.dev.mode == PM_SCAN) { int rc = init_device_state(); if (rc) return rc; }
+      if (cp.dev.mode == PM_SCAN) {
+        int rc = init_device_state();
+        if (rc) return rc;
+        enter_unit(cp.desc && !units.empty() ? units.size() - 1 : 0);
+      }
     }
     cudaEvent_t t0, t1;
     cudaEventCreate(&t0); cudaEventCreate(&t1);
     cudaEventRecord(t0, stream);
     int rc;
-    if (cp.dev.mode == PM_SCAN) rc = cp.desc ? next_scan_batch_desc(scan_rows, out) : next_scan_batch(scan_rows, out);
+    if (cp.dev.mode == PM_SCAN) rc = next_scan_batch(scan_rows, out);
     else if (cp.dev.mode == PM_AGG) rc = run_agg(out);
     else rc = run_topn(out);
     cudaEventRecord(t1, stream);
