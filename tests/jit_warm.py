@@ -31,6 +31,8 @@ def test_plans():
     sc.check_like_known_answers(rec)
     plans += [p for n, p in sc.mixed_plans() if "like" in n or "decimal" in n]
     sc.check_scalar_known_answers(rec, error_labels=("int_divide(-9223372036854775808,-1)", "neg_uint(9223372036854775809)", "abs(-9223372036854775808)"))
+    import test_gpu_group_tables
+    plans += [p for _, p in test_gpu_group_tables.race_plans()]
     for fx in sc.reference_executor_fixtures():
         if fx[0] in ("hash_agg_fast_v2", "topn_integration_3", "topn_unsigned_col0_desc"):
             plans.append(fx[2])

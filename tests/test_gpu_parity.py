@@ -533,18 +533,6 @@ def test_multi_column_group_by(name, plan, jit, regions):
         assert_same_rows(got, exp, ordered=False, float_rel_tol=1e-12 if name == "mg_same_expr_twice" else None, ctx=f"{name}/seed{seed}")
 
 
-@pytest.mark.parametrize("bits", [1, 5])
-def test_multi_column_group_by_hash_collisions(bits, regions, monkeypatch):
-    """Composite-key table with the hash tag cut to a few bits (debug knob): every probe meets equal tags with different
-    keys, inside a warp and across CTAs; results must not change."""
-    monkeypatch.setenv("B2_DEBUG_AGG_HASH_BITS", str(bits))
-    for name, plan in sc.multi_group_plans()[:4]:
-        region = regions[1].build(read_ts=sc.READ_TS, n_write_blocks=2)
-        exp = orc.dag_handle(plan, sc.WHOLE, region)
-        got = DagHandler(plan, sc.WHOLE, DeviceRegion(region), jit=ffi.JIT_OFF).handle_request()
-        assert_same_rows(got, exp, ordered=False, ctx=f"{name}/bits{bits}")
-
-
 def test_multi_column_group_by_generated():
     """Generated table, 200k rows: (a) parity with the oracle for two- and three-column keys incl. a nullable column,
     (b) at 4M rows the group counts add up and the number of groups is the product of the key cardinalities."""

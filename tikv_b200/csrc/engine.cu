@@ -315,6 +315,9 @@ struct b2_exec {
   b2_batch async_batch{};
   bool async_running = false;
   uint64_t paging_size = 0;
+  // B2_DEBUG_AGG_HASH_BITS (read when the request opens): keep only this many bits of the composite-key hash tag, so that
+  // different keys collide in the group table on purpose (tests); 0 = all 64
+  unsigned int debug_hash_bits = 0;
 
   int fail(int status, const std::string& msg, int mysql = 0, uint64_t entry = ~0ull) {
     last_err.status = status; last_err.mysql_code = mysql; last_err.entry_index = entry;
@@ -1363,7 +1366,6 @@ struct b2_exec {
     }
     size_t smem = 0;
     uint32_t smem_slots = 0;
-    static const unsigned int debug_hash_bits = [] { const char* v = getenv("B2_DEBUG_AGG_HASH_BITS"); return v ? (unsigned int)atoi(v) : 0u; }();
     if (P.has_group && P.n_group <= 1) {
       // small on purpose (192 resident groups per CTA): it absorbs the low-cardinality case, where global atomics would
       // serialise on a few addresses; beyond that the HBM table lives in L2 anyway and a big CTA table only costs
@@ -1414,7 +1416,7 @@ struct b2_exec {
       }
       rc = read_counters(&c);
       if (rc) return rc;
-      if (c.agg_overflow && cap < (1u << 30)) {  // group table full: grow and redo (partial results are discarded)
+      if (c.agg_overflow && !c.agg_stuck && cap < (1u << 30)) {  // group table full: grow and redo (partial results are discarded)
         cap <<= 2;
         for (auto& s : slots) s.block = -1;
         continue;
@@ -1423,6 +1425,9 @@ struct b2_exec {
     }
     fill_stats(c);
     drained = true;
+    if (c.agg_stuck)
+      return fail(B2_ERR_UNSUPPORTED, "composite-key group table: " + std::to_string(c.agg_stuck) + " inserts gave up waiting for a claimed slot's key (longest probe run " +
+                                          std::to_string(c.agg_probe_max) + " slots)");
     if (c.agg_overflow) return fail(B2_ERR_UNSUPPORTED, "group table exceeded the device capacity");
     if (c.err != ~0ull) { device_error(c); return publish_agg(0, nullptr, nullptr, nullptr, out); }
     check_trailing_lock();
@@ -1694,6 +1699,7 @@ int32_t b2_exec_open(const b2_dag_plan* plan, const b2_key_range* ranges, uint32
   h->out_loc = cfg ? cfg->output_location : B2_LOC_DEVICE;
   h->deadline_ns = cfg ? cfg->deadline_ns : 0;
   h->paging_size = cfg ? cfg->paging_size : 0;
+  if (const char* v = getenv("B2_DEBUG_AGG_HASH_BITS")) h->debug_hash_bits = (unsigned int)std::min(63, std::max(0, atoi(v)));
   if (h->paging_size && h->cp.dev.mode != PM_SCAN) {
     // Aggregation / TopN under paging depend on the reference's 1024-row batch boundaries (aggr_executor.rs:226-236,
     // top_n_executor.rs:304-318): the CPU executors keep those requests

@@ -29,6 +29,8 @@ struct Counters {
   unsigned long long err_max;          // max over failing rows of (global_entry << 8 | DevErr): the first error of a backward scan; 0 = none
   unsigned long long warn_div0;        // "Division by 0" warnings (1365) raised on committed rows
   unsigned long long first_row;        // smallest global CF_WRITE entry index a row was returned for (take_scanned_range, backward); ~0 = none
+  unsigned int agg_stuck;              // composite-key inserts that gave up waiting for a claimed slot's key (the request fails)
+  unsigned int agg_probe_max;          // longest composite-key probe run above 64 slots (reported with agg_stuck)
 };
 
 // Open-addressing group table in HBM (fast_hash_aggr_executor.rs:216-229 `Groups`): slot = hash(key) & mask, linear
@@ -36,6 +38,7 @@ struct Counters {
 // start at zero and are only added to, so a claimed slot needs no further initialisation).  Slot `cap` is the NULL-key
 // group, slot `cap + 1` the group whose key equals AGG_EMPTY_KEY; `special[0..1]` say whether those two are in use.
 #define AGG_EMPTY_KEY 0xffffffffffffffffull
+#define AGG_MAX_PROBES 4096u  // longest probe run of a key; a longer one counts as a full table (grow and redo)
 struct AggTable {
   unsigned long long* keys;  // cap + 2
   unsigned int* special;     // 2

@@ -29,7 +29,9 @@ __device__ __forceinline__ void st_release_u32(unsigned int* p, unsigned int v) 
 }
 
 // ---- HBM group table ----------------------------------------------------------------------------------
-// returns slot index, or 0xffffffff when the table is full
+// returns slot index, or 0xffffffff when the table is full.  A key probes at most AGG_MAX_PROBES slots (the table has at
+// least 2^16): a run that long only forms in a table close to full, and the engine then grows it and runs the request
+// again.  Without the bound, the inserts after the table fills would each walk the whole table before giving up.
 __device__ unsigned int table_find_or_insert(const AggTable& t, uint64_t key, bool is_null) {
   if (is_null || key == AGG_EMPTY_KEY) {
     const unsigned int which = is_null ? 0u : 1u;
@@ -38,7 +40,7 @@ __device__ unsigned int table_find_or_insert(const AggTable& t, uint64_t key, bo
   }
   unsigned int mask = t.cap - 1;
   unsigned int s = (unsigned int)mix64(key) & mask;
-  for (unsigned int probes = 0; probes < t.cap; ++probes) {
+  for (unsigned int probes = 0; probes < AGG_MAX_PROBES; ++probes) {
     unsigned long long kk = ld_volatile_u64(&t.keys[s]);  // one L2 round trip per probe
     if (kk == AGG_EMPTY_KEY) kk = atomicCAS(&t.keys[s], AGG_EMPTY_KEY, (unsigned long long)key);
     if (kk == AGG_EMPTY_KEY || kk == key) return s;
@@ -49,34 +51,58 @@ __device__ unsigned int table_find_or_insert(const AggTable& t, uint64_t key, bo
 
 // Composite keys (BatchSlowHashAggregation): the table is keyed by a hash tag, claimed with one CAS; the winner then
 // publishes the key words (release on ready[s]); a later arrival with an equal tag waits for them and compares: equal
-// -> same group, different (a 64-bit hash collision) -> keep probing.  `kw` = n_group value words + NULL mask.
-__device__ __forceinline__ unsigned int table_find_or_insert_multi(const AggTable& t, uint64_t tag, const uint64_t (&kw)[MAX_GROUP + 1], int n_words) {
+// -> same group, different (a hash collision) -> keep probing.  `kw` = n_group value words + NULL mask.
+//
+// Called by all lanes `lanes` of one warp together, converged (`want`: this lane has a key to insert), which probe in
+// lock step: every lane takes one probe step, the lanes that claimed a slot publish its key words, the lanes sync, and
+// only then do the lanes that met an equal tag wait for that slot's key.  So no lane ever waits for a warp-mate that has
+// yet to publish, and every wait is on a publisher that is already past its CAS and has nothing left to wait for.  A call
+// still gives up after AGG_POLL_BUDGET reads of `ready` in all its probes (counted in agg_stuck; the engine then fails
+// the request), so that a broken protocol shows up as a failed request rather than as a kernel that does not finish.
+// Returns the slot, or 0xffffffff when the table is full (agg_overflow is set), the call gave up, or !want.
+#define AGG_POLL_BUDGET (1u << 20)
+__device__ __forceinline__ unsigned int table_find_or_insert_multi(const AggTable& t, Counters* ctr, unsigned int lanes, bool want, uint64_t tag,
+                                                                   const uint64_t (&kw)[MAX_GROUP + 1], int n_words) {
   const unsigned int mask = t.cap - 1;
-  unsigned int s = (unsigned int)tag & mask;
-  for (unsigned int probes = 0; probes < t.cap; ++probes) {
-    unsigned long long kk = ld_volatile_u64(&t.keys[s]);
-    if (kk == AGG_EMPTY_KEY) {
-      kk = atomicCAS(&t.keys[s], AGG_EMPTY_KEY, (unsigned long long)tag);
+  unsigned int s = (unsigned int)tag & mask, probes = 0, polls = 0, slot = 0xffffffffu;
+  bool done = !want;
+  do {
+    bool check = false;
+    if (!done) {
+      unsigned long long kk = ld_volatile_u64(&t.keys[s]);
       if (kk == AGG_EMPTY_KEY) {
+        kk = atomicCAS(&t.keys[s], AGG_EMPTY_KEY, (unsigned long long)tag);
+        if (kk == AGG_EMPTY_KEY) {
+#pragma unroll
+          for (int q = 0; q <= MAX_GROUP; ++q)
+            if (q < n_words) t.gkeys[(size_t)s * n_words + q] = kw[q];
+          __threadfence();
+          st_release_u32(&t.ready[s], 1u);
+          slot = s; done = true;
+        }
+      }
+      check = !done && kk == tag;
+    }
+    __syncwarp(lanes);  // the claims of this step are published
+    if (check) {
+      bool published = false;
+      while (!(published = ld_acquire_u32(&t.ready[s]) != 0) && ++polls < AGG_POLL_BUDGET) {}
+      if (!published) { atomicAdd(&ctr->agg_stuck, 1u); done = true; }
+      else {
+        bool same = true;
 #pragma unroll
         for (int q = 0; q <= MAX_GROUP; ++q)
-          if (q < n_words) t.gkeys[(size_t)s * n_words + q] = kw[q];
-        __threadfence();
-        st_release_u32(&t.ready[s], 1u);
-        return s;
+          if (q < n_words) same = same && ld_volatile_u64(&t.gkeys[(size_t)s * n_words + q]) == kw[q];
+        if (same) { slot = s; done = true; }
       }
     }
-    if (kk == tag) {
-      while (ld_acquire_u32(&t.ready[s]) == 0) {}
-      bool same = true;
-#pragma unroll
-      for (int q = 0; q <= MAX_GROUP; ++q)
-        if (q < n_words) same = same && ld_volatile_u64(&t.gkeys[(size_t)s * n_words + q]) == kw[q];
-      if (same) return s;
+    if (!done) {
+      s = (s + 1) & mask;
+      if (++probes == AGG_MAX_PROBES) { atomicExch(&ctr->agg_overflow, 1u); done = true; }
     }
-    s = (s + 1) & mask;
-  }
-  return 0xffffffffu;
+  } while (!__all_sync(lanes, done));
+  if (probes > 64) atomicMax(&ctr->agg_probe_max, probes);  // (a healthy table at most half full stays far below)
+  return slot;
 }
 
 // barrier over the 256 row-decoding threads only (the scan kernel runs a 9th, producer-only warp)
@@ -811,10 +837,15 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
           const int lead = __ffs(peers) - 1;
           if (__popc(__ballot_sync(active, lead == (int)lane)) > 28) peers = 1u << lane;  // (nearly) one group per lane
           else {
+            // every lane of `peers` takes part in every shuffle: a `same && __shfl_sync(..)` would skip the shuffles of a
+            // lane that already differs, and its warp-mates would wait for it (equal tags, different keys)
             bool same = true;
 #pragma unroll
             for (int q = 0; q <= MAX_GROUP; ++q)
-              if (q <= P.n_group) same = same && __shfl_sync(peers, gw[q], lead) == gw[q];
+              if (q <= P.n_group) {
+                const uint64_t lw = __shfl_sync(peers, gw[q], lead);
+                same = same && lw == gw[q];
+              }
             if (__any_sync(active, !same)) peers = 1u << lane;  // equal tags, different keys inside the warp: no pre-aggregation
           }
         } else if (P.has_group) {
@@ -828,11 +859,11 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
         const bool leader = (unsigned int)(__ffs(peers) - 1) == lane;
         const bool solo = (peers & (peers - 1)) == 0;
         unsigned long long* acc = nullptr;
+        // (all lanes of `active` take part, so that none of them waits at another warp-synchronous instruction meanwhile)
+        const unsigned int mslot = MODE == PM_AGGM ? table_find_or_insert_multi(A.tbl, A.ctr, active, leader, gk.bits, gw, P.n_group + 1) : 0xffffffffu;
         if (leader) {
           if (MODE == PM_AGGM) {
-            unsigned int gslot = table_find_or_insert_multi(A.tbl, gk.bits, gw, P.n_group + 1);
-            if (gslot == 0xffffffffu) atomicExch(&A.ctr->agg_overflow, 1u);
-            else acc = A.tbl.acc + (size_t)gslot * P.acc_words;
+            if (mslot != 0xffffffffu) acc = A.tbl.acc + (size_t)mslot * P.acc_words;
           } else if (!P.has_group) acc = s_simple_acc;
           else {
             if (st.slots && !s_tbl_off && !gk.null && gk.bits != SMEM_EMPTY_KEY) {
