@@ -99,6 +99,11 @@ typedef struct b2_cf_block {
 /* kvrpcpb::IsolationLevel */
 enum { B2_ISO_SI = 0, B2_ISO_RC = 1, B2_ISO_RC_CHECK_TS = 2 };
 
+/* B2_LOC_DEVICE blocks must be complete when the request opens (b2_exec_open, b2_dag_handle, b2_checksum_handle): the
+ * engine reads them on its own stream (b2_exec_config.cuda_stream or a non-blocking stream it creates) and does not
+ * order itself behind other streams, the legacy default stream included.  A producer that writes the blocks
+ * asynchronously synchronises (or makes cuda_stream wait on its work) before the call.  b2_gen_create, b2_sst_decode and
+ * b2_region_pin return with their blocks complete. */
 typedef struct b2_region_source {
   int32_t location;              /* of write/default blocks; lock block is always host memory */
   int32_t device;                /* CUDA ordinal for B2_LOC_DEVICE pointers / where to run */
@@ -266,7 +271,8 @@ typedef struct b2_dag_plan {
 typedef struct b2_exec_config {
   int32_t output_location;  /* B2_LOC_HOST: results copied to host memory; B2_LOC_DEVICE: device ptrs */
   int32_t staging_tiles;    /* 0 = default */
-  uint64_t cuda_stream;     /* 0 = handle creates its own stream; else a cudaStream_t to run on */
+  uint64_t cuda_stream;     /* 0 = handle creates its own stream; else a cudaStream_t to run on (device-resident blocks
+                             * must be complete when the request opens: see b2_region_source) */
   int32_t jit;              /* plan-specialised kernel (compiled at run time, cached per plan): B2_JIT_AUTO = background
                              * compile for large requests and switch when ready, B2_JIT_SYNC = wait for it at open,
                              * B2_JIT_OFF = always the generic kernel.  Environment B2_JIT=auto|sync|off overrides.

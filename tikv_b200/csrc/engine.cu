@@ -107,6 +107,33 @@ struct BufPool {
 BufPool& dev_pool() { static BufPool p(false, 24ull << 30); return p; }
 BufPool& host_pool() { static BufPool p(true, 8ull << 30); return p; }
 
+// Timing events, reused across requests (per process, per device): creating and destroying them costs a driver call each,
+// and a request times every launch.  An event taken from the pool has completed whatever it last recorded, because
+// a request waits for its stream before giving its events back.
+struct EventPool {
+  std::mutex mu;
+  std::vector<std::pair<int, cudaEvent_t>> free_list;
+  cudaEvent_t get() {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    {
+      std::lock_guard<std::mutex> g(mu);
+      for (size_t i = free_list.size(); i-- > 0;)
+        if (free_list[i].first == dev) { cudaEvent_t e = free_list[i].second; free_list.erase(free_list.begin() + i); return e; }
+    }
+    cudaEvent_t e = nullptr;
+    return cudaEventCreate(&e) == cudaSuccess ? e : nullptr;
+  }
+  void put(cudaEvent_t e) {  // the event's device must be current
+    if (!e) return;
+    int dev = 0;
+    cudaGetDevice(&dev);
+    std::lock_guard<std::mutex> g(mu);
+    free_list.push_back({dev, e});
+  }
+};
+EventPool& event_pool() { static EventPool* p = new EventPool(); return *p; }
+
 // A block taken from `Pool` and owned: it goes back to the pool when the buffer is destroyed or released, moving leaves the
 // source empty.  The pool tags a returned block with the current device, so that device must be current then.
 template <BufPool& (*Pool)()>
@@ -290,7 +317,7 @@ struct b2_exec {
   std::vector<DevBuf> res_cols, res_bitmaps;
   unsigned int tbl_cap = 0;
   StageSlot slots[2];
-  HostBuf h_out, h_ctr;
+  HostBuf h_out, h_ctr, h_res_ptrs;
   uint64_t out_cap = 0;
 
   // results exposed through b2_batch
@@ -337,18 +364,17 @@ struct b2_exec {
       if (s.ready) cudaEventDestroy(s.ready);
       if (s.free_ev) cudaEventDestroy(s.free_ev);
     }
-    for (auto& e : kev) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
+    for (auto& e : kev) { event_pool().put(e.first); event_pool().put(e.second); }
+    for (cudaEvent_t e : batch_ev) event_pool().put(e);
     if (own_stream && stream) cudaStreamDestroy(stream);
   }
-  // the handle's streams: kernels run on the caller's stream (cfg->cuda_stream) or an own one, block staging on an own one
+  // the handle's streams: kernels run on the caller's stream (cfg->cuda_stream) or an own one; block staging of host
+  // sources on an own one, created when the first block is staged
   cudaError_t open_streams(const b2_exec_config* cfg) {
-    if (cfg && cfg->cuda_stream) stream = (cudaStream_t)cfg->cuda_stream;
-    else {
-      cudaError_t e = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
-      if (e != cudaSuccess) return e;
-      own_stream = true;
-    }
-    return cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking);
+    if (cfg && cfg->cuda_stream) { stream = (cudaStream_t)cfg->cuda_stream; return cudaSuccess; }
+    cudaError_t e = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
+    if (e == cudaSuccess) own_stream = true;
+    return e;
   }
 
   Counters* ctr() { return (Counters*)ctr_buf.p; }
@@ -380,19 +406,24 @@ struct b2_exec {
 
   // Row format of the first row a unit will touch (TiDB tables are all-v1 or all-v2 in practice); decides whether the
   // v1 twin of the exact-layout path is part of the kernel.  A wrong guess only costs speed: every row is checked.
+  // (A device source's first value was read by compute_units.)
+  uint32_t v1_sample_len = 0;
+  uint8_t v1_sample[48];
   bool sample_is_v1() {
     if (units.empty()) return false;
-    const Unit& u = units[0];
-    const SrcBlock& b = wblocks[u.block_idx];
-    if (u.e_lo >= b.c.n) return false;
-    uint32_t off[2];
     uint8_t buf[64];
     memset(buf, 0, sizeof(buf));
-    if (src_loc == B2_LOC_HOST) { off[0] = b.c.val_offs[u.e_lo]; off[1] = b.c.val_offs[u.e_lo + 1]; }
-    else if (cudaMemcpy(off, b.c.val_offs + u.e_lo, 8, cudaMemcpyDeviceToHost) != cudaSuccess) return false;
-    uint32_t n = std::min<uint32_t>(off[1] - off[0], 48);
-    if (src_loc == B2_LOC_HOST) memcpy(buf, b.c.vals + off[0], n);
-    else if (cudaMemcpy(buf, b.c.vals + off[0], n, cudaMemcpyDeviceToHost) != cudaSuccess) return false;
+    uint32_t n;
+    if (src_loc == B2_LOC_HOST) {
+      const Unit& u = units[0];
+      const SrcBlock& b = wblocks[u.block_idx];
+      if (u.e_lo >= b.c.n) return false;
+      n = std::min<uint32_t>(b.c.val_offs[u.e_lo + 1] - b.c.val_offs[u.e_lo], 48);
+      memcpy(buf, b.c.vals + b.c.val_offs[u.e_lo], n);
+    } else {
+      n = std::min<uint32_t>(v1_sample_len, 48);
+      memcpy(buf, v1_sample, n);
+    }
     // write record: type, varint start_ts, then 'v' len row... (write.rs:296-361); anything else: no opinion
     uint32_t pos = 1;
     while (pos < n && (buf[pos] & 0x80)) ++pos;
@@ -402,39 +433,34 @@ struct b2_exec {
   }
 
   // ---- source setup ----
-  int read_offs_end(const b2_cf_block& b, uint64_t* kb, uint64_t* vb) {
-    uint32_t k = 0, v = 0;
-    if (b.n == 0) { *kb = *vb = 0; return B2_OK; }
-    if (src_loc == B2_LOC_HOST) { k = b.key_offs[b.n]; v = b.val_offs[b.n]; }
-    else {
-      CUDA_TRY(cudaMemcpy(&k, b.key_offs + b.n, 4, cudaMemcpyDeviceToHost));
-      CUDA_TRY(cudaMemcpy(&v, b.val_offs + b.n, 4, cudaMemcpyDeviceToHost));
-    }
-    *kb = k; *vb = v;
-    return B2_OK;
+  static void host_offs_end(const b2_cf_block& b, uint64_t* kb, uint64_t* vb) {
+    *kb = b.n ? b.key_offs[b.n] : 0;
+    *vb = b.n ? b.val_offs[b.n] : 0;
   }
 
+  // A device-resident source is read once while the request opens (compute_units): heap sizes, range bounds, unit
+  // prefixes and the row-format sample come back in one copy, behind one stream synchronise.
   int setup_source(const b2_region_source* src, const b2_key_range* ranges, uint32_t n_ranges) {
     src_loc = src->location;
     read_ts = src->read_ts; isolation = src->isolation_level; check_newer = src->check_has_newer_ts_data != 0;
+    const bool host = src_loc == B2_LOC_HOST;
     uint64_t base = 0;
     for (uint32_t i = 0; i < src->n_write; ++i) {
       SrcBlock sb; sb.c = src->write[i]; sb.entry_base = base;
-      int rc = read_offs_end(sb.c, &sb.key_bytes, &sb.val_bytes);
-      if (rc) return rc;
+      if (host) host_offs_end(sb.c, &sb.key_bytes, &sb.val_bytes);
       base += sb.c.n;
       wblocks.push_back(sb);
     }
     for (uint32_t i = 0; src->dflt && i < src->n_dflt; ++i) {
       SrcBlock sb; sb.c = src->dflt[i];
-      int rc = read_offs_end(sb.c, &sb.key_bytes, &sb.val_bytes);
-      if (rc) return rc;
+      if (host) host_offs_end(sb.c, &sb.key_bytes, &sb.val_bytes);
       dblocks.push_back(sb);
     }
-    // CF_DEFAULT views on the device (host sources are copied once; long values are rare)
-    if (!dblocks.empty()) {
+    // CF_DEFAULT views of a host source on the device: its blocks are copied once (long values are rare).  A device source's
+    // views are written by compute_units.
+    if (!dblocks.empty() && host) {
       std::vector<BlockView> views;
-      if (src_loc == B2_LOC_HOST) {
+      {
         size_t total = 0;
         for (auto& d : dblocks) total += ((d.key_bytes + 31) & ~15ull) + ((d.val_bytes + 31) & ~15ull) + 2 * (((size_t)d.c.n + 1) * 4 + 16);
         CUDA_TRY(dflt_store.reserve(total));
@@ -453,8 +479,6 @@ struct b2_exec {
           v.voff = (const uint32_t*)put(d.c.val_offs, ((size_t)d.c.n + 1) * 4);
           views.push_back(v);
         }
-      } else {
-        for (auto& d : dblocks) { BlockView v; v.keys = d.c.keys; v.koff = d.c.key_offs; v.vals = d.c.vals; v.voff = d.c.val_offs; v.n = d.c.n; views.push_back(v); }
       }
       CUDA_TRY(dflt_views.reserve(views.size() * sizeof(BlockView)));
       CUDA_TRY(cudaMemcpyAsync(dflt_views.p, views.data(), views.size() * sizeof(BlockView), cudaMemcpyHostToDevice, stream));
@@ -528,12 +552,67 @@ struct b2_exec {
     return compute_units();
   }
 
+  // Device source: one upload (block views, range bounds), the probe kernels, one download into pinned memory, one wait.
+  // Fills res / unit_ok (compute_units' layout), the heap sizes of every block, the CF_DEFAULT views and the v1 sample.
+  HostBuf h_open;
+  int probe_device_source(uint32_t* res, uint32_t* unit_ok) {
+    const uint32_t nr = (uint32_t)range_lo.size(), nb = (uint32_t)wblocks.size(), nd = (uint32_t)dblocks.size();
+    if (!nb && !nd) return B2_OK;
+    auto a16 = [](size_t n) { return (n + 15) & ~(size_t)15; };
+    size_t flat_bytes = 0;
+    for (uint32_t r = 0; r < nr; ++r) flat_bytes += range_lo[r].size() + range_hi[r].size();
+    const size_t views_at = 0, flat_at = a16((size_t)(nb + nd) * sizeof(BlockView)), offs_at = flat_at + a16(flat_bytes + 16);
+    const size_t in_bytes = a16(offs_at + ((size_t)nr * 2 + 1) * 4);
+    const size_t n_ends = 2 * (size_t)(nb + nd), n_res = (size_t)nb * nr * 2, n_ok = (size_t)nb * nr * 4, n_sample = 1 + 12;
+    const size_t out_bytes = (n_ends + n_res + n_ok + n_sample) * 4;
+    CUDA_TRY(h_open.reserve(in_bytes + out_bytes));
+    DevBuf d_open;
+    CUDA_TRY(d_open.reserve(in_bytes + out_bytes));
+    uint8_t* h = (uint8_t*)h_open.p;
+    BlockView* views = (BlockView*)(h + views_at);
+    for (uint32_t i = 0; i < nb + nd; ++i) {
+      const b2_cf_block& c = i < nb ? wblocks[i].c : dblocks[i - nb].c;
+      views[i].keys = c.keys; views[i].koff = c.key_offs; views[i].vals = c.vals; views[i].voff = c.val_offs; views[i].n = c.n;
+    }
+    uint8_t* flat = h + flat_at;
+    uint32_t* offs = (uint32_t*)(h + offs_at);
+    offs[0] = 0;
+    size_t at = 0;
+    for (uint32_t r = 0; r < nr; ++r) {
+      memcpy(flat + at, range_lo[r].data(), range_lo[r].size()); at += range_lo[r].size(); offs[2 * r + 1] = (uint32_t)at;
+      memcpy(flat + at, range_hi[r].data(), range_hi[r].size()); at += range_hi[r].size(); offs[2 * r + 2] = (uint32_t)at;
+    }
+    uint8_t* d = (uint8_t*)d_open.p;
+    uint32_t* d_out = (uint32_t*)(d + in_bytes);
+    cudaError_t e = cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, stream);
+    if (e == cudaSuccess)
+      e = launch_open_probe((const BlockView*)(d + views_at), nb, nb + nd, d + flat_at, (const uint32_t*)(d + offs_at), nr, first_live_range, d_out + n_ends,
+                            d_out + n_ends + n_res, d_out, d_out + n_ends + n_res + n_ok, stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h + in_bytes, d_out, out_bytes, cudaMemcpyDeviceToHost, stream);
+    if (e == cudaSuccess && nd) e = dflt_views.reserve((size_t)nd * sizeof(BlockView));
+    if (e == cudaSuccess && nd) e = cudaMemcpyAsync(dflt_views.p, d + views_at + (size_t)nb * sizeof(BlockView), (size_t)nd * sizeof(BlockView), cudaMemcpyDeviceToDevice, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) return fail(B2_ERR_CUDA, std::string("opening the request's blocks: ") + cudaGetErrorString(e));
+    const uint32_t* out = (const uint32_t*)(h + in_bytes);
+    for (uint32_t i = 0; i < nb + nd; ++i) {
+      SrcBlock& sb = i < nb ? wblocks[i] : dblocks[i - nb];
+      sb.key_bytes = out[2 * i]; sb.val_bytes = out[2 * i + 1];
+    }
+    memcpy(res, out + n_ends, n_res * 4);
+    memcpy(unit_ok, out + n_ends + n_res, n_ok * 4);
+    v1_sample_len = out[n_ends + n_res + n_ok];
+    memcpy(v1_sample, out + n_ends + n_res + n_ok + 1, sizeof(v1_sample));
+    return B2_OK;
+  }
+
   // lower_bound of every range bound in every CF_WRITE block
   int compute_units() {
     uint32_t nr = (uint32_t)range_lo.size(), nb = (uint32_t)wblocks.size();
-    if (!nr || !nb) return B2_OK;
     std::vector<uint32_t> res((size_t)nb * nr * 2), unit_ok((size_t)nb * nr * 4, 0);  // unit_ok: [ok, 12 prefix bytes] per (block, range)
-    if (src_loc == B2_LOC_HOST) {
+    if (src_loc != B2_LOC_HOST) {
+      int rc = probe_device_source(res.data(), unit_ok.data());
+      if (rc) return rc;
+    } else if (nr && nb) {
       for (uint32_t b = 0; b < nb; ++b)
         for (uint32_t q = 0; q < nr * 2; ++q) {
           const std::vector<uint8_t>& key = (q & 1) ? range_hi[q / 2] : range_lo[q / 2];
@@ -555,29 +634,6 @@ struct b2_exec {
           unit_ok[((size_t)b * nr + r) * 4] = ok;
           if (ok) memcpy(&unit_ok[((size_t)b * nr + r) * 4 + 1], f, 12);
         }
-    } else {
-      std::vector<uint8_t> flat;
-      std::vector<uint32_t> offs(1, 0);
-      for (uint32_t r = 0; r < nr; ++r) {
-        flat.insert(flat.end(), range_lo[r].begin(), range_lo[r].end()); offs.push_back((uint32_t)flat.size());
-        flat.insert(flat.end(), range_hi[r].begin(), range_hi[r].end()); offs.push_back((uint32_t)flat.size());
-      }
-      std::vector<BlockView> views;
-      for (auto& w : wblocks) { BlockView v; v.keys = w.c.keys; v.koff = w.c.key_offs; v.vals = w.c.vals; v.voff = w.c.val_offs; v.n = w.c.n; views.push_back(v); }
-      DevBuf d_views, d_flat, d_offs, d_res, d_ok;
-      cudaError_t e = d_views.reserve(views.size() * sizeof(BlockView));
-      if (e == cudaSuccess) e = d_ok.reserve(unit_ok.size() * 4);
-      if (e == cudaSuccess) e = d_flat.reserve(flat.size() + 16);
-      if (e == cudaSuccess) e = d_offs.reserve(offs.size() * 4);
-      if (e == cudaSuccess) e = d_res.reserve(res.size() * 4);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(d_views.p, views.data(), views.size() * sizeof(BlockView), cudaMemcpyHostToDevice, stream);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(d_flat.p, flat.data(), flat.size(), cudaMemcpyHostToDevice, stream);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(d_offs.p, offs.data(), offs.size() * 4, cudaMemcpyHostToDevice, stream);
-      if (e == cudaSuccess) e = launch_bounds_search((const BlockView*)d_views.p, nb, (const uint8_t*)d_flat.p, (const uint32_t*)d_offs.p, nr * 2, (uint32_t*)d_res.p, (uint32_t*)d_ok.p, stream);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(res.data(), d_res.p, res.size() * 4, cudaMemcpyDeviceToHost, stream);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(unit_ok.data(), d_ok.p, unit_ok.size() * 4, cudaMemcpyDeviceToHost, stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-      if (e != cudaSuccess) return fail(B2_ERR_CUDA, std::string("range bounds search: ") + cudaGetErrorString(e));
     }
     for (uint32_t r = first_live_range; r < nr; ++r)
       for (uint32_t b = 0; b < nb; ++b) {
@@ -608,6 +664,7 @@ struct b2_exec {
     const SrcBlock& sb = wblocks[bi];
     // pick the slot not holding the previous block (two slots alternate)
     StageSlot* s = &slots[bi & 1];
+    if (!copy_stream) CUDA_TRY(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
     if (!s->ready) { CUDA_TRY(cudaEventCreateWithFlags(&s->ready, cudaEventDisableTiming)); CUDA_TRY(cudaEventCreateWithFlags(&s->free_ev, cudaEventDisableTiming)); }
     if (s->free_recorded) CUDA_TRY(cudaStreamWaitEvent(copy_stream, s->free_ev, 0));
     size_t kb = (sb.key_bytes + 31) & ~15ull, vb = (sb.val_bytes + 31) & ~15ull, ob = ((size_t)sb.c.n + 1) * 4;
@@ -660,18 +717,32 @@ struct b2_exec {
 
   int init_device_state() {
     CUDA_TRY(ctr_buf.reserve(sizeof(Counters)));
-    CUDA_TRY(h_ctr.reserve(sizeof(Counters)));
+    CUDA_TRY(h_ctr.reserve(2 * sizeof(Counters)));
     memset(&good_ctr, 0, sizeof(good_ctr));
     good_ctr.err = ~0ull; good_ctr.first_row = ~0ull;
-    CUDA_TRY(cudaMemcpyAsync(ctr_buf.p, &good_ctr, sizeof(good_ctr), cudaMemcpyHostToDevice, stream));
+    int rc = upload_counters(good_ctr);
+    if (rc) return rc;
     CUDA_TRY(range_rows.reserve(std::max<size_t>(1, range_raw_lo.size()) * 8));
     CUDA_TRY(cudaMemsetAsync(range_rows.p, 0, std::max<size_t>(1, range_raw_lo.size()) * 8, stream));
     range_rows_taken.assign(range_raw_lo.size(), 0);
     return B2_OK;
   }
+  // h_ctr holds two Counters: [0] receives read_counters, [1] is the pinned source of this upload.  The source may only be
+  // rewritten once the previous upload has been waited for (read_counters), else the copy could read the new bytes:
+  // a second upload before that is a bug in the engine and fails the request instead of racing.
+  bool ctr_upload_in_flight = false;
+  int upload_counters(const Counters& c) {
+    if (ctr_upload_in_flight) return fail(B2_ERR_CUDA, "internal: counters uploaded again before the previous upload was waited for");
+    Counters* src = (Counters*)h_ctr.p + 1;
+    *src = c;
+    CUDA_TRY(cudaMemcpyAsync(ctr_buf.p, src, sizeof(Counters), cudaMemcpyHostToDevice, stream));
+    ctr_upload_in_flight = true;
+    return B2_OK;
+  }
   int read_counters(Counters* c) {
     CUDA_TRY(cudaMemcpyAsync(h_ctr.p, ctr_buf.p, sizeof(Counters), cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
+    ctr_upload_in_flight = false;
     memcpy(c, h_ctr.p, sizeof(Counters));
     harvest_kernel_times();
     return B2_OK;
@@ -679,12 +750,9 @@ struct b2_exec {
   // CUDA events bracketing every launch of the dominant kernel (roofline numerator / denominator in bench.py)
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> kev;
   size_t kev_used = 0;
+  cudaEvent_t batch_ev[2] = {nullptr, nullptr};  // brackets each next_batch (time_processed_ns)
   void kernel_begin() {
-    if (kev_used == kev.size()) {
-      cudaEvent_t a, b;
-      cudaEventCreate(&a); cudaEventCreate(&b);
-      kev.push_back({a, b});
-    }
+    if (kev_used == kev.size()) kev.push_back({event_pool().get(), event_pool().get()});
     cudaEventRecord(kev[kev_used].first, stream);
   }
   void kernel_end() { cudaEventRecord(kev[kev_used].second, stream); ++kev_used; stats.kernel_launches++; }
@@ -993,7 +1061,8 @@ struct b2_exec {
         // were returned (the reference's partial-result semantics)
         const Counters bad = c;
         cur_unit = save_unit; cur_lo = save_lo; cur_hi = save_hi; entries_scanned = save_scanned;
-        CUDA_TRY(cudaMemcpyAsync(ctr_buf.p, &good_ctr, sizeof(good_ctr), cudaMemcpyHostToDevice, stream));
+        rc = upload_counters(good_ctr);
+        if (rc) return rc;
         CUDA_TRY(cudaMemcpyAsync(range_rows.p, range_rows_prev.p, rr_bytes, cudaMemcpyDeviceToDevice, stream));
         rc = run_scan_pass(budget, first_error(bad) >> 8, &lock_r, &c);
         if (rc) return rc;
@@ -1414,6 +1483,15 @@ struct b2_exec {
         entries_scanned += u.e_hi - u.e_lo;
         stats.num_iterations++;
       }
+      // the group table -> compact group list right behind the last unit, so that one read of the counters serves both;
+      // the list of a table that overflowed is discarded with it
+      if (P.has_group) {
+        size_t W = P.acc_words;
+        CUDA_TRY(grp_keys.reserve(((size_t)tbl_cap + 2) * 8 * std::max(1, P.n_group))); CUDA_TRY(grp_null.reserve((size_t)tbl_cap + 2)); CUDA_TRY(grp_acc.reserve(((size_t)tbl_cap + 2) * 8 * W));
+        AggTable t; t.keys = (unsigned long long*)tbl_keys.p; t.special = (unsigned int*)tbl_occ.p; t.acc = (unsigned long long*)tbl_acc.p; t.cap = tbl_cap;
+        t.gkeys = (unsigned long long*)tbl_gkeys.p; t.ready = (unsigned int*)tbl_ready.p; t.hash_mask_bits = 0;
+        CUDA_TRY(launch_agg_finalize(P, t, ctr(), (unsigned long long*)grp_keys.p, (unsigned char*)grp_null.p, (unsigned long long*)grp_acc.p, stream));
+      }
       rc = read_counters(&c);
       if (rc) return rc;
       if (c.agg_overflow && !c.agg_stuck && cap < (1u << 30)) {  // group table full: grow and redo (partial results are discarded)
@@ -1439,13 +1517,6 @@ struct b2_exec {
       n_groups = c.live_rows > 0 ? 1 : 0;  // simple_aggr_executor.rs:141-148, 233-248
       ga = (const unsigned long long*)tbl_acc.p;
     } else {
-      size_t W = P.acc_words;
-      CUDA_TRY(grp_keys.reserve(((size_t)tbl_cap + 2) * 8 * std::max(1, P.n_group))); CUDA_TRY(grp_null.reserve((size_t)tbl_cap + 2)); CUDA_TRY(grp_acc.reserve(((size_t)tbl_cap + 2) * 8 * W));
-      AggTable t; t.keys = (unsigned long long*)tbl_keys.p; t.special = (unsigned int*)tbl_occ.p; t.acc = (unsigned long long*)tbl_acc.p; t.cap = tbl_cap;
-      t.gkeys = (unsigned long long*)tbl_gkeys.p; t.ready = (unsigned int*)tbl_ready.p; t.hash_mask_bits = 0;
-      CUDA_TRY(launch_agg_finalize(P, t, ctr(), (unsigned long long*)grp_keys.p, (unsigned char*)grp_null.p, (unsigned long long*)grp_acc.p, stream));
-      int rc = read_counters(&c);
-      if (rc) return rc;
       n_groups = c.n_groups;
       gk = (const unsigned long long*)grp_keys.p; gn = (const unsigned char*)grp_null.p; ga = (const unsigned long long*)grp_acc.p;
     }
@@ -1469,9 +1540,11 @@ struct b2_exec {
       CUDA_TRY(cudaMemsetAsync(res_bitmaps[k].p, 0xff, std::max<size_t>(8, bm_bytes), stream));
       ptrs[k] = res_cols[k].p; ptrs[ncol + k] = res_bitmaps[k].p;
     }
-    if (n_groups) {
+    if (n_groups) {  // (one publish per request: the pinned source is written once)
       CUDA_TRY(res_ptrs.reserve(ptrs.size() * sizeof(void*)));
-      CUDA_TRY(cudaMemcpyAsync(res_ptrs.p, ptrs.data(), ptrs.size() * sizeof(void*), cudaMemcpyHostToDevice, stream));
+      CUDA_TRY(h_res_ptrs.reserve(ptrs.size() * sizeof(void*)));
+      memcpy(h_res_ptrs.p, ptrs.data(), ptrs.size() * sizeof(void*));
+      CUDA_TRY(cudaMemcpyAsync(res_ptrs.p, h_res_ptrs.p, ptrs.size() * sizeof(void*), cudaMemcpyHostToDevice, stream));
       CUDA_TRY(launch_agg_result(P, n_groups, gk, gn, ga, (unsigned long long**)res_ptrs.p, (unsigned long long**)res_ptrs.p + ncol, stream));
     }
     // deliver the requested output offsets
@@ -1483,7 +1556,7 @@ struct b2_exec {
     }
     int rc = publish_fixed(fc, n_groups);
     if (rc) return rc;
-    CUDA_TRY(cudaStreamSynchronize(stream));
+    // (next_batch waits for the stream before it returns the batch)
     out->columns = cols.data(); out->n_columns = (uint32_t)n_out; out->n_rows = n_groups; out->n_warnings = 0;
     out->is_drained = B2_DRAIN_DRAINED;
     stats.num_produced_rows += n_groups;
@@ -1639,8 +1712,8 @@ struct b2_exec {
         enter_unit(cp.desc && !units.empty() ? units.size() - 1 : 0);
       }
     }
-    cudaEvent_t t0, t1;
-    cudaEventCreate(&t0); cudaEventCreate(&t1);
+    if (!batch_ev[0]) { batch_ev[0] = event_pool().get(); batch_ev[1] = event_pool().get(); }
+    cudaEvent_t t0 = batch_ev[0], t1 = batch_ev[1];
     cudaEventRecord(t0, stream);
     int rc;
     if (cp.dev.mode == PM_SCAN) rc = next_scan_batch(scan_rows, out);
@@ -1651,7 +1724,6 @@ struct b2_exec {
     float ms = 0;
     cudaEventElapsedTime(&ms, t0, t1);
     stats.time_processed_ns += (uint64_t)(ms * 1e6);
-    cudaEventDestroy(t0); cudaEventDestroy(t1);
     out->n_warnings = (uint32_t)std::min<uint64_t>(warnings_total - warnings_reported, 0xffffffffull);
     warnings_reported = warnings_total;
     return rc;
@@ -1710,8 +1782,8 @@ int32_t b2_exec_open(const b2_dag_plan* plan, const b2_key_range* ranges, uint32
   h->cp.dev.isolation = src->isolation_level;
   if (!h->cp.pool.empty()) {  // bytes constants (LIKE patterns): to HBM, their launch parameters become cell references into it
     e = h->const_pool.reserve(h->cp.pool.size() + 16);
+    // (no wait: the source lives as long as the handle, and the kernels that read the copy run behind it on the same stream)
     if (e == cudaSuccess) e = cudaMemcpyAsync(h->const_pool.p, h->cp.pool.data(), h->cp.pool.size(), cudaMemcpyHostToDevice, h->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
     if (e != cudaSuccess) { g_last_error = std::string("bytes constants: ") + cudaGetErrorString(e); return B2_ERR_CUDA; }
     patch_pool_imms(h->cp, (const uint8_t*)h->const_pool.p);
   }

@@ -387,19 +387,27 @@ cudaError_t launch_agg_result(const DevPlan& plan, unsigned int n_groups, const 
 
 
 // ---- range bounds: lower_bound of each encoded key in each block -------------------------------------------
+// One warp per (block, bound), 33-way: each round the 32 lanes compare 32 evenly spaced keys, so a 3e7-entry block takes
+// 5 rounds of dependent HBM reads instead of 25 (the request waits for this search before its first unit starts).
+// Invariant: every entry below lo is < the bound, every entry at or above hi is >= it.
 __global__ void bounds_kernel(const BlockView* blocks, uint32_t n_blocks, const uint8_t* bounds, const uint32_t* bound_offs, uint32_t n_bounds, uint32_t* out) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_blocks * n_bounds) return;
-  uint32_t bi = i / n_bounds, qi = i % n_bounds;
+  const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (i >= n_blocks * n_bounds) return;  // (warp-uniform)
+  const uint32_t bi = i / n_bounds, qi = i % n_bounds;
   const BlockView b = blocks[bi];
   const uint8_t* q = bounds + bound_offs[qi];
-  uint32_t qn = bound_offs[qi + 1] - bound_offs[qi];
+  const uint32_t qn = bound_offs[qi + 1] - bound_offs[qi];
+  auto less = [&](uint32_t e) { return bytes_cmp(b.keys + b.koff[e], b.koff[e + 1] - b.koff[e], q, qn) < 0; };
   uint32_t lo = 0, hi = b.n;
-  while (lo < hi) {
-    uint32_t mid = lo + (hi - lo) / 2;
-    if (bytes_cmp(b.keys + b.koff[mid], b.koff[mid + 1] - b.koff[mid], q, qn) < 0) lo = mid + 1; else hi = mid;
+  while (hi - lo > 32) {
+    const uint32_t p = lo + (uint32_t)(((unsigned long long)(hi - lo) * (lane + 1)) / 33);  // strictly increasing in lane, < hi
+    const uint32_t c = __popc(__ballot_sync(0xffffffffu, less(p)));                         // keys below the bound form a prefix
+    const uint32_t p_below = __shfl_sync(0xffffffffu, p, c ? c - 1 : 0), p_at = __shfl_sync(0xffffffffu, p, c < 32 ? c : 31);
+    if (c) lo = p_below + 1;
+    if (c < 32) hi = p_at;
   }
-  out[i] = lo;
+  const uint32_t c = __popc(__ballot_sync(0xffffffffu, lo + lane < hi && less(lo + lane)));
+  if (lane == 0) out[i] = lo + c;
 }
 
 // per (block, range) unit [lo, hi): do its first and last key share their first 12 bytes, and are those the start of a
@@ -422,12 +430,39 @@ __global__ void unit_prefix_kernel(const BlockView* blocks, uint32_t n_blocks, u
   out[4 * i] = ok;
 }
 
-cudaError_t launch_bounds_search(const BlockView* blocks, uint32_t n_blocks, const uint8_t* bounds, const uint32_t* bound_offs, uint32_t n_bounds,
-                                 uint32_t* out, uint32_t* unit_ok, cudaStream_t s) {
-  uint32_t n = n_blocks * n_bounds;
-  if (!n) return cudaSuccess;
-  bounds_kernel<<<(n + 63) / 64, 64, 0, s>>>(blocks, n_blocks, bounds, bound_offs, n_bounds, out);
-  unit_prefix_kernel<<<(n / 2 + 63) / 64, 64, 0, s>>>(blocks, n_blocks, n_bounds / 2, out, unit_ok);
+// ends: per block (the n_wblocks CF_WRITE blocks, then the CF_DEFAULT ones) its key and value heap sizes, key_offs[n] and
+// val_offs[n].  sample: byte count, then up to 48 bytes of the first value of the first unit (ranges from first_range on,
+// in the order the host builds units), which tells the host the row format.
+__global__ void block_ends_kernel(const BlockView* blocks, uint32_t n_wblocks, uint32_t n_blocks, uint32_t n_ranges, uint32_t first_range,
+                                  const uint32_t* bounds, uint32_t* ends, uint32_t* sample) {
+  for (uint32_t b = threadIdx.x; b < n_blocks; b += blockDim.x) {
+    const BlockView v = blocks[b];
+    ends[2 * b] = v.n ? v.koff[v.n] : 0u;
+    ends[2 * b + 1] = v.n ? v.voff[v.n] : 0u;
+  }
+  if (threadIdx.x) return;
+  sample[0] = 0;
+  for (uint32_t r = first_range; r < n_ranges; ++r)
+    for (uint32_t b = 0; b < n_wblocks; ++b) {
+      const uint32_t lo = bounds[(size_t)b * n_ranges * 2 + 2 * r], hi = bounds[(size_t)b * n_ranges * 2 + 2 * r + 1];
+      if (hi <= lo) continue;
+      const BlockView v = blocks[b];
+      const uint32_t o = v.voff[lo], n = min(v.voff[lo + 1] - o, 48u);
+      uint8_t* dst = reinterpret_cast<uint8_t*>(sample + 1);
+      for (uint32_t j = 0; j < n; ++j) dst[j] = v.vals[o + j];
+      sample[0] = n;
+      return;
+    }
+}
+
+cudaError_t launch_open_probe(const BlockView* blocks, uint32_t n_wblocks, uint32_t n_blocks, const uint8_t* bounds, const uint32_t* bound_offs, uint32_t n_ranges,
+                              uint32_t first_range, uint32_t* out, uint32_t* unit_ok, uint32_t* ends, uint32_t* sample, cudaStream_t s) {
+  const uint32_t n = n_wblocks * n_ranges * 2;
+  if (n) {
+    bounds_kernel<<<(n + 3) / 4, 128, 0, s>>>(blocks, n_wblocks, bounds, bound_offs, n_ranges * 2, out);
+    unit_prefix_kernel<<<(n / 2 + 63) / 64, 64, 0, s>>>(blocks, n_wblocks, n_ranges, out, unit_ok);
+  }
+  block_ends_kernel<<<1, 128, 0, s>>>(blocks, n_wblocks, n_blocks, n ? n_ranges : 0, first_range, out, ends, sample);
   return cudaGetLastError();
 }
 

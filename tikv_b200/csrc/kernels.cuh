@@ -145,9 +145,12 @@ cudaError_t launch_topn_merge2(const DevPlan& plan, const TopItem* a, const unsi
                                unsigned int* out_cnt, uint32_t limit, cudaStream_t s);
 cudaError_t launch_pack_nulls(const unsigned char* nulls, uint32_t n_cols, uint32_t stride, uint32_t n, unsigned long long* bitmaps, uint32_t words_per_col, cudaStream_t s);
 size_t topn_smem_bytes(uint32_t cap, int n_order);
-// out: lower_bound of every bound in every block; unit_ok[block * n_ranges + range]: that unit's keys share a record-key prefix
-cudaError_t launch_bounds_search(const BlockView* blocks, uint32_t n_blocks, const uint8_t* bounds, const uint32_t* bound_offs, uint32_t n_bounds,
-                                 uint32_t* out, uint32_t* unit_ok, cudaStream_t s);
+// What opening a request over device-resident blocks reads from them.  blocks: the n_wblocks CF_WRITE blocks, then the
+// CF_DEFAULT ones (n_blocks in all).  out: lower_bound of every range bound (lo, hi per range) in every CF_WRITE block;
+// unit_ok[block * n_ranges + range]: that unit's keys share a record-key prefix; ends: key_offs[n], val_offs[n] per block;
+// sample: the byte count and first bytes of the first value of the first unit of the ranges from first_range on
+cudaError_t launch_open_probe(const BlockView* blocks, uint32_t n_wblocks, uint32_t n_blocks, const uint8_t* bounds, const uint32_t* bound_offs, uint32_t n_ranges,
+                              uint32_t first_range, uint32_t* out, uint32_t* unit_ok, uint32_t* ends, uint32_t* sample, cudaStream_t s);
 cudaError_t launch_gen_sizes(const b2_gen_spec& spec, uint32_t* row_entries, uint32_t* row_val_bytes, cudaStream_t s);
 cudaError_t launch_gen_write(const GenArgs& a, cudaStream_t s);
 cudaError_t launch_fill_u64(unsigned long long* p, unsigned long long v, size_t n, cudaStream_t s);
