@@ -222,7 +222,11 @@ typedef struct b2_rpn_expr {
 
 /* tipb::ExprType aggregate kinds (tidb_query_aggr/src/parser.rs:67-88) */
 enum { B2_AGG_COUNT = 3001, B2_AGG_SUM = 3002, B2_AGG_AVG = 3003, B2_AGG_MIN = 3004,
-       B2_AGG_MAX = 3005, B2_AGG_FIRST = 3006 };
+       B2_AGG_MAX = 3005, B2_AGG_FIRST = 3006,
+       /* Agg_BitAnd / Agg_BitOr / Agg_BitXor over an Int argument (a Real argument is B2_ERR_UNSUPPORTED: no Real->Int
+        * cast here).  The output column is B2_COL_I64, B2_TP_LONGLONG, UNSIGNED | NOT_NULL, the type TiDB infers for them
+        * (b2_aggr_desc carries no output field type).  FIRST outputs one column of its argument's type, NOT_NULL cleared. */
+       B2_AGG_BIT_AND = 3008, B2_AGG_BIT_OR = 3009, B2_AGG_BIT_XOR = 3010 };
 
 typedef struct b2_aggr_desc {
   int32_t kind;      /* B2_AGG_* */
@@ -434,7 +438,13 @@ void b2_exec_close(b2_exec* h);
  *   COUNT: [count]   SUM/AVG over Int: [count, sum of low 32 bits, sum of high 32 bits]
  *   SUM/AVG over Real: [count, 66 words]: the exact sum as a 2112-bit fixed-point number (bit 0 = 2^-1074), one signed
  *   32-bit digit per word, carry-save; partial sums merge by word-wise integer addition and round once at the end
- *   MAX/MIN: [count, extremum key]: the key merges by unsigned 64-bit maximum (bit w of max_word_mask marks such words) */
+ *   MAX/MIN: [count, extremum key]: the key merges by unsigned 64-bit maximum (bit w of max_word_mask marks such words)
+ *   BIT_OR: [bits], merges by OR   BIT_XOR: [bits], merges by XOR   BIT_AND: [OR of the complemented inputs], merges by
+ *   OR; the result is ~bits
+ *   FIRST: [key, value] at an even word (padding words before it are additive zeros): the pair with the larger key wins;
+ *   key 0 = no row, bit 0 of the key = the value is NULL.  Keys order the rows of one request only: a merge across
+ *   requests takes the first request, in scan order, whose key is nonzero
+ * b2_exec_agg_word_ops tells how each word merges. */
 typedef struct b2_agg_partials {
   uint32_t n_groups;
   uint32_t acc_words;
@@ -448,6 +458,10 @@ typedef struct b2_agg_partials {
   uint32_t _pad;
 } b2_agg_partials;
 int32_t b2_exec_agg_partials(b2_exec* h, b2_agg_partials* out);
+/* How each word of b2_agg_partials.acc merges: ops[w] = B2_MERGE_*, w < acc_words.  Valid whenever b2_exec_agg_partials
+ * is.  *n_inout: capacity of `ops` in, acc_words out (B2_ERR_INVALID_ARG when the capacity is smaller). */
+enum { B2_MERGE_ADD = 0, B2_MERGE_MAX = 1, B2_MERGE_OR = 2, B2_MERGE_XOR = 3, B2_MERGE_FIRST_KEY = 4, B2_MERGE_FIRST_VALUE = 5 };
+int32_t b2_exec_agg_word_ops(b2_exec* h, uint8_t* ops, uint32_t* n_inout);
 
 /* RequestHandler::handle_request for a DAG: run to drain.  Result columns are owned by *out_handle
  * (close it with b2_exec_close). */

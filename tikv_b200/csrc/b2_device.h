@@ -94,7 +94,8 @@ struct DevNode {
   int64_t imm;  // const bits (i64 or f64 bits) or column offset
 };
 struct DevExpr { uint16_t start, n; };
-struct DevAgg { DevExpr arg; uint8_t kind /*0 count 1 sum 2 avg 3 max 4 min*/, arg_et, arg_unsigned, acc_off; };
+enum AggKind { AGG_COUNT = 0, AGG_SUM = 1, AGG_AVG = 2, AGG_MAX = 3, AGG_MIN = 4, AGG_FIRST = 5, AGG_BIT_AND = 6, AGG_BIT_OR = 7, AGG_BIT_XOR = 8 };
+struct DevAgg { DevExpr arg; uint8_t kind /*AggKind*/, arg_et, arg_unsigned, acc_off; };
 struct DevOrder { DevExpr e; uint8_t desc, et, is_unsigned, _pad; };
 
 enum PlanMode { PM_SCAN = 0, PM_AGG = 1, PM_TOPN = 2, PM_CHECKSUM = 3,
@@ -2079,6 +2080,67 @@ B2_HD uint64_t extremum_value(uint64_t key, int arg_et, bool arg_unsigned, bool 
   if (arg_et == 1) return (k >> 63) ? (k & 0x7fffffffffffffffull) : ~k;
   return arg_unsigned ? k : (k ^ 0x8000000000000000ull);
 }
+
+// FIRST / BIT_AND / BIT_OR / BIT_XOR state.  Every state is all-zero words before its first row, like the others.
+//   BIT_OR  [bits]: |= v          BIT_XOR [bits]: ^= v          BIT_AND [bits]: |= ~v, the result is ~bits
+//   FIRST   [key, value] at an even word: the pair with the larger key wins (128-bit compare-and-swap); key 0 = no row
+// (impl_bit_op.rs BitOp::init_state / AggrFnStateBitOp::update_concrete: NULL inputs are skipped, the state starts at
+// !0 / 0 / 0; impl_first.rs AggrFnStateFirst::update: the first row's value, NULL included)
+B2_HD bool agg_is_extremum(int kind) { return kind == AGG_MAX || kind == AGG_MIN; }
+B2_HD bool agg_is_bit(int kind) { return kind >= AGG_BIT_AND; }
+// the word a BIT_* row contributes (0 for NULL: the identity of OR and XOR)
+B2_HD uint64_t bit_agg_word(int kind, bool has, uint64_t bits) { return !has ? 0ull : (kind == AGG_BIT_AND ? ~bits : bits); }
+// FIRST's key of the row at block entry `entry`: 2^63 | ((2^62 - 1 - r) << 1) | is_null, where r is the row's rank in scan
+// order.  It is the TopN tie rule (`desc ? ~entry : entry`): ranges arrive ascending and non-overlapping, so entries rise in
+// a forward scan and fall in a backward one.  A larger key is a row scanned earlier; the lean kernel and the list-mode
+// kernel commit different rows of one unit and must agree on this key.
+B2_HD uint64_t first_agg_key(uint64_t entry, bool desc, bool is_null) {
+  const uint64_t r62 = (1ull << 62) - 1, r = desc ? r62 - entry : entry;
+  return (1ull << 63) | ((r62 - r) << 1) | (is_null ? 1ull : 0ull);
+}
+// one row into a FIRST / BIT_* state, sequentially (what the kernels' pre-aggregation and atomics compute)
+B2_HD void first_bit_update(int kind, uint64_t* w, uint64_t entry, bool desc, bool has, uint64_t bits) {
+  if (kind == AGG_FIRST) {
+    const uint64_t key = first_agg_key(entry, desc, !has);
+    if (key > w[0]) { w[0] = key; w[1] = has ? bits : 0ull; }
+  } else if (kind == AGG_BIT_XOR) w[0] ^= bit_agg_word(kind, has, bits);
+  else w[0] |= bit_agg_word(kind, has, bits);
+}
+// the result cell of a FIRST / BIT_* state; false = NULL (FIRST without a row, or whose first row's value is NULL)
+B2_HD bool first_bit_result(int kind, const uint64_t* w, uint64_t* out) {
+  if (kind == AGG_FIRST) {
+    const bool has = w[0] != 0 && !(w[0] & 1);
+    *out = has ? w[1] : 0ull;
+    return has;
+  }
+  *out = kind == AGG_BIT_AND ? ~w[0] : w[0];
+  return true;
+}
+// how a word of the accumulator state merges (b2_exec_agg_word_ops); the FIRST value word follows its key word
+B2_HD int agg_word_op(const DevPlan& P, int w) {
+  for (int a = 0; a < P.n_aggs; ++a) {
+    const DevAgg& g = P.aggs[a];
+    if (agg_is_extremum(g.kind) && w == g.acc_off + 1) return B2_MERGE_MAX;
+    if ((g.kind == AGG_BIT_AND || g.kind == AGG_BIT_OR) && w == g.acc_off) return B2_MERGE_OR;
+    if (g.kind == AGG_BIT_XOR && w == g.acc_off) return B2_MERGE_XOR;
+    if (g.kind == AGG_FIRST && w == g.acc_off) return B2_MERGE_FIRST_KEY;
+    if (g.kind == AGG_FIRST && w == g.acc_off + 1) return B2_MERGE_FIRST_VALUE;
+  }
+  return B2_MERGE_ADD;  // counts, integer limbs, the digits of exact Real sums and alignment padding
+}
+#ifdef __CUDACC__
+// FIRST: store (key, value) at `w` (16-byte aligned, shared or global) unless the stored key is at least as large
+__device__ __forceinline__ void first_agg_update(unsigned long long* w, unsigned long long key, unsigned long long value) {
+  unsigned long long lo = *(volatile unsigned long long*)&w[0];
+  while (key > lo) {
+    unsigned long long hi = *(volatile unsigned long long*)&w[1];
+    const unsigned long long want_lo = lo, want_hi = hi;
+    asm volatile("{\n\t.reg .b128 d, c, s;\n\tmov.b128 c, {%0, %1};\n\tmov.b128 s, {%2, %3};\n\tatom.cas.b128 d, [%4], c, s;\n\tmov.b128 {%0, %1}, d;\n\t}"
+                 : "+l"(lo), "+l"(hi) : "l"(key), "l"(value), "l"(w) : "memory");
+    if (lo == want_lo && hi == want_hi) break;
+  }
+}
+#endif
 
 // one output cell of a PM_SCAN pipeline: a scan column (LazyBatchColumn::ensure_decoded) or, under a Projection
 // (projection_executor.rs:199-222), the value of its `oc`-th selected expression

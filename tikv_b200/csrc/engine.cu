@@ -1896,7 +1896,16 @@ int32_t b2_exec_agg_partials(b2_exec* h, b2_agg_partials* out) {
   out->max_word_mask = 0;
   out->key_words = (uint32_t)std::max(1, h->cp.dev.n_group); out->_pad = 0;
   for (int a = 0; a < h->cp.dev.n_aggs; ++a)
-    if (h->cp.dev.aggs[a].kind >= 3) out->max_word_mask |= 1ull << (h->cp.dev.aggs[a].acc_off + 1);
+    if (agg_is_extremum(h->cp.dev.aggs[a].kind)) out->max_word_mask |= 1ull << (h->cp.dev.aggs[a].acc_off + 1);
+  return B2_OK;
+}
+int32_t b2_exec_agg_word_ops(b2_exec* h, uint8_t* ops, uint32_t* n_inout) {
+  if (!h || !ops || !n_inout) { g_last_error = "null argument"; return B2_ERR_INVALID_ARG; }
+  if (h->cp.dev.mode != PM_AGG || !h->drained) { g_last_error = "no aggregation state: not an Aggregation pipeline or not drained yet"; return B2_ERR_INVALID_ARG; }
+  const uint32_t n = (uint32_t)h->cp.dev.acc_words;
+  if (*n_inout < n) { *n_inout = n; g_last_error = "ops buffer smaller than acc_words"; return B2_ERR_INVALID_ARG; }
+  for (uint32_t w = 0; w < n; ++w) ops[w] = (uint8_t)agg_word_op(h->cp.dev, (int)w);
+  *n_inout = n;
   return B2_OK;
 }
 

@@ -271,10 +271,16 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
               const DevAgg g = P.aggs[a];
               const bool has = !av[a].null;
               r_cnt[a] += has ? 1u : 0u;
-              if (g.kind >= 3) {
-                const unsigned long long key = has ? extremum_key(av[a].bits, g.arg_et, g.arg_unsigned, g.kind == 4) : 0ull;
+              if (agg_is_extremum(g.kind)) {
+                const unsigned long long key = has ? extremum_key(av[a].bits, g.arg_et, g.arg_unsigned, g.kind == AGG_MIN) : 0ull;
                 r_lo[a] = key > r_lo[a] ? key : r_lo[a];
-              } else if (g.kind != 0 && has) {
+              } else if (g.kind == AGG_FIRST) {  // r_lo / r_hi: the lane's (key, value) pair
+                const unsigned long long key = first_agg_key(A.entry_base + e, A.desc, !has);
+                if (key > r_lo[a]) { r_lo[a] = key; r_hi[a] = has ? av[a].bits : 0ull; }
+              } else if (agg_is_bit(g.kind)) {
+                const unsigned long long x = bit_agg_word(g.kind, has, av[a].bits);
+                r_lo[a] = g.kind == AGG_BIT_XOR ? r_lo[a] ^ x : r_lo[a] | x;
+              } else if (g.kind != AGG_COUNT && has) {
                 r_lo[a] += (uint32_t)av[a].bits;
                 r_hi[a] += g.arg_unsigned ? (unsigned long long)(uint32_t)(av[a].bits >> 32) : (unsigned long long)(long long)(int32_t)(av[a].bits >> 32);
               }
@@ -314,16 +320,32 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
               const unsigned int cnt = solo ? (has ? 1u : 0u) : __reduce_add_sync(peers, has ? 1u : 0u);
               unsigned long long* w = acc + g.acc_off;
               const bool commit_w = leader && acc != nullptr && cnt != 0;
-              if (g.kind == 0) {
+              if (g.kind == AGG_COUNT) {
                 if (commit_w) atomicAdd(&w[0], (unsigned long long)cnt);
-              } else if (g.kind >= 3) {
-                unsigned long long key = has ? extremum_key(av[a].bits, g.arg_et, g.arg_unsigned, g.kind == 4) : 0ull;
+              } else if (agg_is_extremum(g.kind)) {
+                unsigned long long key = has ? extremum_key(av[a].bits, g.arg_et, g.arg_unsigned, g.kind == AGG_MIN) : 0ull;
                 if (!solo)
                   for (unsigned int mm = peers & (peers - 1); mm; mm &= mm - 1) {
                     unsigned long long other = __shfl_sync(peers, key, __ffs(mm) - 1);
                     key = other > key ? other : key;
                   }
                 if (commit_w) { atomicAdd(&w[0], (unsigned long long)cnt); atomicMax(&w[1], key); }
+              } else if (g.kind == AGG_FIRST) {
+                unsigned long long key = first_agg_key(A.entry_base + e, A.desc, !has), val = has ? av[a].bits : 0ull;
+                if (!solo)
+                  for (unsigned int mm = peers & (peers - 1); mm; mm &= mm - 1) {
+                    const unsigned long long ok2 = __shfl_sync(peers, key, __ffs(mm) - 1), ov = __shfl_sync(peers, val, __ffs(mm) - 1);
+                    if (ok2 > key) { key = ok2; val = ov; }
+                  }
+                if (leader && acc != nullptr) first_agg_update(w, key, val);
+              } else if (agg_is_bit(g.kind)) {
+                unsigned long long x = bit_agg_word(g.kind, has, av[a].bits);
+                if (!solo) {
+                  const unsigned int lo = g.kind == AGG_BIT_XOR ? __reduce_xor_sync(peers, (unsigned int)x) : __reduce_or_sync(peers, (unsigned int)x);
+                  const unsigned int hi = g.kind == AGG_BIT_XOR ? __reduce_xor_sync(peers, (unsigned int)(x >> 32)) : __reduce_or_sync(peers, (unsigned int)(x >> 32));
+                  x = ((unsigned long long)hi << 32) | lo;
+                }
+                if (leader && acc != nullptr && x) { if (g.kind == AGG_BIT_XOR) atomicXor(&w[0], x); else atomicOr(&w[0], x); }
               } else {
                 const uint32_t lo = has ? (uint32_t)av[a].bits : 0u, hi = has ? (uint32_t)(av[a].bits >> 32) : 0u;
                 unsigned long long lo_sum, hi_sum;
@@ -428,15 +450,21 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
           const DevAgg g = P.aggs[a];
           for (int off = 16; off > 0; off >>= 1) {
             r_cnt[a] += __shfl_xor_sync(0xffffffffu, r_cnt[a], off);
-            const unsigned long long o_lo = __shfl_xor_sync(0xffffffffu, r_lo[a], off);
-            if (g.kind >= 3) r_lo[a] = o_lo > r_lo[a] ? o_lo : r_lo[a]; else r_lo[a] += o_lo;
-            r_hi[a] += __shfl_xor_sync(0xffffffffu, r_hi[a], off);
+            const unsigned long long o_lo = __shfl_xor_sync(0xffffffffu, r_lo[a], off), o_hi = __shfl_xor_sync(0xffffffffu, r_hi[a], off);
+            if (agg_is_extremum(g.kind)) r_lo[a] = o_lo > r_lo[a] ? o_lo : r_lo[a];
+            else if (g.kind == AGG_FIRST) { if (o_lo > r_lo[a]) { r_lo[a] = o_lo; r_hi[a] = o_hi; } }
+            else if (g.kind == AGG_BIT_XOR) r_lo[a] ^= o_lo;
+            else if (agg_is_bit(g.kind)) r_lo[a] |= o_lo;
+            else r_lo[a] += o_lo;
+            if (g.kind != AGG_FIRST) r_hi[a] += o_hi;
           }
-          if (lane == 0 && r_cnt[a]) {
-            unsigned long long* w = A.tbl.acc + g.acc_off;
+          unsigned long long* w = A.tbl.acc + g.acc_off;
+          if (lane == 0 && g.kind == AGG_FIRST && r_lo[a]) first_agg_update(w, r_lo[a], r_hi[a]);
+          else if (lane == 0 && agg_is_bit(g.kind) && r_lo[a]) { if (g.kind == AGG_BIT_XOR) atomicXor(&w[0], r_lo[a]); else atomicOr(&w[0], r_lo[a]); }
+          else if (lane == 0 && r_cnt[a] && g.kind < AGG_FIRST) {
             atomicAdd(&w[0], r_cnt[a]);
-            if (g.kind >= 3) atomicMax(&w[1], r_lo[a]);
-            else if (g.kind != 0) { atomicAdd(&w[1], r_lo[a]); atomicAdd(&w[2], r_hi[a]); }
+            if (agg_is_extremum(g.kind)) atomicMax(&w[1], r_lo[a]);
+            else if (g.kind != AGG_COUNT) { atomicAdd(&w[1], r_lo[a]); atomicAdd(&w[2], r_hi[a]); }
           }
         }
       }
@@ -451,9 +479,11 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
           const unsigned long long* src = st.acc + (size_t)s * P.acc_words + g.acc_off;
           unsigned long long* dst = A.tbl.acc + (size_t)gslot * P.acc_words + g.acc_off;
           if (src[0] == 0) continue;
+          if (g.kind == AGG_FIRST) { first_agg_update(dst, src[0], src[1]); continue; }
+          if (agg_is_bit(g.kind)) { if (g.kind == AGG_BIT_XOR) atomicXor(&dst[0], src[0]); else atomicOr(&dst[0], src[0]); continue; }
           atomicAdd(&dst[0], src[0]);
-          if (g.kind == 0) continue;
-          if (g.kind >= 3) atomicMax(&dst[1], src[1]);
+          if (g.kind == AGG_COUNT) continue;
+          if (agg_is_extremum(g.kind)) atomicMax(&dst[1], src[1]);
           else { atomicAdd(&dst[1], src[1]); atomicAdd(&dst[2], src[2]); }
         }
       }

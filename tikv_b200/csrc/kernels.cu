@@ -359,10 +359,18 @@ __global__ void agg_result_kernel(const __grid_constant__ DevPlan P, unsigned in
       if (!has) atomicAnd(&col_bitmap[c][g >> 6], ~(1ull << (g & 63)));
       ++c;
     }
-    if (ag.kind == 3 || ag.kind == 4) {  // MAX / MIN: NULL without a non-NULL input
+    if (agg_is_extremum(ag.kind)) {  // MAX / MIN: NULL without a non-NULL input
       bool has = cnt != 0;
-      col_data[c][g] = has ? extremum_value(acc[ag.acc_off + 1], ag.arg_et, ag.arg_unsigned, ag.kind == 4) : 0ull;
+      col_data[c][g] = has ? extremum_value(acc[ag.acc_off + 1], ag.arg_et, ag.arg_unsigned, ag.kind == AGG_MIN) : 0ull;
       if (!has) atomicAnd(&col_bitmap[c][g >> 6], ~(1ull << (g & 63)));
+      ++c;
+    }
+    // FIRST: NULL without a row or when the first row's value is NULL (impl_first.rs AggrFnStateFirst::push_result);
+    // BIT_*: never NULL (impl_bit_op.rs AggrFnStateBitOp::push_result)
+    if (ag.kind == AGG_FIRST || agg_is_bit(ag.kind)) {
+      uint64_t v;
+      if (!first_bit_result(ag.kind, (const uint64_t*)acc + ag.acc_off, &v)) atomicAnd(&col_bitmap[c][g >> 6], ~(1ull << (g & 63)));
+      col_data[c][g] = v;
       ++c;
     }
   }

@@ -396,29 +396,49 @@ inline int compile_plan(const b2_dag_plan* plan, CompiledPlan* out, std::string*
       P.mode = PM_AGG; terminal = true;
       schema.clear();
       int acc = 0;
+      bool has_first = false;
       for (uint32_t k = 0; k < e.n_aggrs; ++k) {
         DevAgg& g = P.aggs[k];
         int tp; uint32_t flag; uint8_t et, uns;
+        const int ak = e.aggrs[k].kind;
+        const bool bit_op = ak == B2_AGG_BIT_AND || ak == B2_AGG_BIT_OR || ak == B2_AGG_BIT_XOR;
+        if ((ak == B2_AGG_FIRST || bit_op) && e.aggrs[k].arg.n_nodes) {  // (the argument's type: its root node, the last in post-order)
+          const int ck = scan_col_kind(e.aggrs[k].arg.nodes[e.aggrs[k].arg.n_nodes - 1].field_tp, 0);
+          if (ck >= CK_TIME && ck <= CK_DEC) {
+            *msg = ak == B2_AGG_FIRST ? "FIRST over a bytes / JSON / decimal / date-time / duration value is not on the device path yet"
+                                      : "BIT_AND / BIT_OR / BIT_XOR over a bytes / JSON / decimal / date-time / duration value (cast to Int) is not supported";
+            return B2_ERR_UNSUPPORTED;
+          }
+        }
         if (!lower_expr(e.aggrs[k].arg, P, &g.arg, &et, &uns, &tp, &flag, msg)) return B2_ERR_UNSUPPORTED;
         g.arg_et = et; g.arg_unsigned = uns;
+        if (ak == B2_AGG_FIRST) acc += acc & 1;  // FIRST's [key, value] pair is one 16-byte compare-and-swap
         g.acc_off = (uint8_t)acc;
         switch (e.aggrs[k].kind) {
-          case B2_AGG_COUNT: g.kind = 0; acc += 1; break;
-          case B2_AGG_SUM: g.kind = 1; acc += et ? 1 + F64_ACC_DIGITS : 3; break;  // Real: exact fixed-point accumulator (b2_device.h f64_acc_add)
-          case B2_AGG_AVG: g.kind = 2; acc += et ? 1 + F64_ACC_DIGITS : 3; break;
-          case B2_AGG_MAX: g.kind = 3; acc += 2; break;
-          case B2_AGG_MIN: g.kind = 4; acc += 2; break;
+          case B2_AGG_COUNT: g.kind = AGG_COUNT; acc += 1; break;
+          case B2_AGG_SUM: g.kind = AGG_SUM; acc += et ? 1 + F64_ACC_DIGITS : 3; break;  // Real: exact fixed-point accumulator (b2_device.h f64_acc_add)
+          case B2_AGG_AVG: g.kind = AGG_AVG; acc += et ? 1 + F64_ACC_DIGITS : 3; break;
+          case B2_AGG_MAX: g.kind = AGG_MAX; acc += 2; break;
+          case B2_AGG_MIN: g.kind = AGG_MIN; acc += 2; break;
+          case B2_AGG_FIRST: g.kind = AGG_FIRST; acc += 2; has_first = true; break;
+          case B2_AGG_BIT_AND: g.kind = AGG_BIT_AND; acc += 1; break;
+          case B2_AGG_BIT_OR: g.kind = AGG_BIT_OR; acc += 1; break;
+          case B2_AGG_BIT_XOR: g.kind = AGG_BIT_XOR; acc += 1; break;
           default: *msg = "aggregate function " + std::to_string(e.aggrs[k].kind) + " is not on the device path yet"; return B2_ERR_UNSUPPORTED;
         }
-        if ((g.kind == 1 || g.kind == 2) && !et && tp == B2_TP_BIT) { *msg = "SUM/AVG over BIT (cast to DOUBLE) is not supported"; return B2_ERR_UNSUPPORTED; }
+        if ((g.kind == AGG_SUM || g.kind == AGG_AVG) && !et && tp == B2_TP_BIT) { *msg = "SUM/AVG over BIT (cast to DOUBLE) is not supported"; return B2_ERR_UNSUPPORTED; }
+        if (agg_is_bit(g.kind) && et == 1) { *msg = "BIT_AND / BIT_OR / BIT_XOR over a Real value (cast to Int) is not supported"; return B2_ERR_UNSUPPORTED; }
         if (acc > MAX_ACC_WORDS) { *msg = "aggregate state too large"; return B2_ERR_UNSUPPORTED; }
         OutCol cnt = {B2_COL_I64, B2_TP_LONGLONG, B2_FLAG_UNSIGNED | B2_FLAG_NOT_NULL};  // impl_count.rs:35-40
         OutCol sum = et ? OutCol{B2_COL_F64, B2_TP_DOUBLE, 0} : OutCol{B2_COL_DECIMAL, B2_TP_NEWDECIMAL, 0};
-        if (g.kind == 0 || g.kind == 2) schema.push_back(cnt);
-        if (g.kind == 1 || g.kind == 2) schema.push_back(sum);
-        if (g.kind == 3 || g.kind == 4)  // one column of the argument's own type (impl_max_min.rs:78-84)
+        if (g.kind == AGG_COUNT || g.kind == AGG_AVG) schema.push_back(cnt);
+        if (g.kind == AGG_SUM || g.kind == AGG_AVG) schema.push_back(sum);
+        if (agg_is_extremum(g.kind) || g.kind == AGG_FIRST)  // one column of the argument's own type (impl_max_min.rs:78-84, impl_first.rs AggrFnStateFirst::push_result)
           schema.push_back(OutCol{et ? B2_COL_F64 : B2_COL_I64, tp, flag & ~(uint32_t)B2_FLAG_NOT_NULL});
+        if (agg_is_bit(g.kind)) schema.push_back(cnt);  // u64, never NULL (include/b2_copr.h B2_AGG_BIT_AND)
       }
+      acc += has_first ? acc & 1 : 0;  // CTA and HBM tables then hold every group's state 16-byte aligned
+      if (acc > MAX_ACC_WORDS) { *msg = "aggregate state too large"; return B2_ERR_UNSUPPORTED; }
       P.n_aggs = (int)e.n_aggrs; P.acc_words = acc;
       if (e.n_group_by == 1) {
         int tp; uint32_t flag; uint8_t et, uns;

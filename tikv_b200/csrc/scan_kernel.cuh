@@ -482,7 +482,7 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
   unsigned long long t_live = 0;
   unsigned int t_first = 0xffffffffu;  // smallest block entry index a row was returned for
   // no-group aggregation: one accumulator set per CTA in shared memory, flushed at the end
-  __shared__ unsigned long long s_simple_acc[MODE == PM_AGG ? MAX_ACC_WORDS : 1];
+  __shared__ __align__(16) unsigned long long s_simple_acc[MODE == PM_AGG ? MAX_ACC_WORDS : 1];  // (FIRST: 16-byte pairs)
   if (MODE == PM_AGG) {
     for (unsigned int i = tid; i < MAX_ACC_WORDS; i += blockDim.x) s_simple_acc[i] = 0;
   }
@@ -899,16 +899,32 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
           const unsigned int cnt = solo ? (has ? 1u : 0u) : __reduce_add_sync(peers, has ? 1u : 0u);
           unsigned long long* w = acc + g.acc_off;  // only dereferenced by a leader that found a slot
           const bool commit = leader && acc != nullptr && cnt != 0;
-          if (g.kind == 0) {
+          if (g.kind == AGG_COUNT) {
             if (commit) atomicAdd(&w[0], (unsigned long long)cnt);
-          } else if (g.kind >= 3) {  // MAX / MIN: running unsigned maximum of the (complemented) order-preserving key
-            unsigned long long key = has ? extremum_key(v.bits, g.arg_et, g.arg_unsigned, g.kind == 4) : 0ull;
+          } else if (agg_is_extremum(g.kind)) {  // MAX / MIN: running unsigned maximum of the (complemented) order-preserving key
+            unsigned long long key = has ? extremum_key(v.bits, g.arg_et, g.arg_unsigned, g.kind == AGG_MIN) : 0ull;
             if (!solo)
               for (unsigned int mm = peers & (peers - 1); mm; mm &= mm - 1) {  // the leader is the lowest lane
                 unsigned long long other = __shfl_sync(peers, key, __ffs(mm) - 1);
                 key = other > key ? other : key;
               }
             if (commit) { atomicAdd(&w[0], (unsigned long long)cnt); atomicMax(&w[1], key); }
+          } else if (g.kind == AGG_FIRST) {  // every row counts, a NULL one too: the peers' earliest (key, value)
+            unsigned long long key = err2 ? 0ull : first_agg_key(A.entry_base + e, A.desc, v.null), val = has ? v.bits : 0ull;
+            if (!solo)
+              for (unsigned int mm = peers & (peers - 1); mm; mm &= mm - 1) {
+                const unsigned long long ok2 = __shfl_sync(peers, key, __ffs(mm) - 1), ov = __shfl_sync(peers, val, __ffs(mm) - 1);
+                if (ok2 > key) { key = ok2; val = ov; }
+              }
+            if (leader && acc != nullptr && key) first_agg_update(w, key, val);
+          } else if (agg_is_bit(g.kind)) {
+            unsigned long long x = bit_agg_word(g.kind, has, v.bits);
+            if (!solo) {
+              const unsigned int lo = g.kind == AGG_BIT_XOR ? __reduce_xor_sync(peers, (unsigned int)x) : __reduce_or_sync(peers, (unsigned int)x);
+              const unsigned int hi = g.kind == AGG_BIT_XOR ? __reduce_xor_sync(peers, (unsigned int)(x >> 32)) : __reduce_or_sync(peers, (unsigned int)(x >> 32));
+              x = ((unsigned long long)hi << 32) | lo;
+            }
+            if (leader && acc != nullptr && x) { if (g.kind == AGG_BIT_XOR) atomicXor(&w[0], x); else atomicOr(&w[0], x); }
           } else if (g.arg_et == 1) {
             // exact: every lane adds its own value into the group's fixed-point accumulator (plans with a Real SUM / AVG run
             // without warp pre-aggregation: `peers` is the lane itself, see above)
@@ -988,12 +1004,14 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
     if (!P.has_group) {
       cta256_sync();
       for (int w = (int)tid; w < P.acc_words; w += TILE) {
-        bool is_max = false;
-        for (int a = 0; a < P.n_aggs; ++a)
-          if (P.aggs[a].kind >= 3 && P.aggs[a].acc_off + 1 == w) is_max = true;
+        const int op = agg_word_op(P, w);
         unsigned long long x = s_simple_acc[w];
-        if (is_max) { if (x) atomicMax(&A.tbl.acc[w], x); }
-        else if (x) atomicAdd(&A.tbl.acc[w], x);  // counts, integer limbs and the digits of exact Real sums are all additive
+        if (!x) continue;  // every state word starts at 0, the identity of its merge
+        if (op == B2_MERGE_MAX) atomicMax(&A.tbl.acc[w], x);
+        else if (op == B2_MERGE_OR) atomicOr(&A.tbl.acc[w], x);
+        else if (op == B2_MERGE_XOR) atomicXor(&A.tbl.acc[w], x);
+        else if (op == B2_MERGE_FIRST_KEY) first_agg_update(&A.tbl.acc[w], x, s_simple_acc[w + 1]);
+        else if (op == B2_MERGE_ADD) atomicAdd(&A.tbl.acc[w], x);  // counts, integer limbs and the digits of exact Real sums are all additive
       }
     } else if (st.slots) {
       cta256_sync();
@@ -1006,9 +1024,11 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
           const unsigned long long* src = st.acc + (size_t)s * P.acc_words + g.acc_off;
           unsigned long long* dst = A.tbl.acc + (size_t)gslot * P.acc_words + g.acc_off;
           if (src[0] == 0) continue;
+          if (g.kind == AGG_FIRST) { first_agg_update(dst, src[0], src[1]); continue; }
+          if (agg_is_bit(g.kind)) { if (g.kind == AGG_BIT_XOR) atomicXor(&dst[0], src[0]); else atomicOr(&dst[0], src[0]); continue; }
           atomicAdd(&dst[0], src[0]);
-          if (g.kind == 0) continue;
-          if (g.kind >= 3) atomicMax(&dst[1], src[1]);
+          if (g.kind == AGG_COUNT) continue;
+          if (agg_is_extremum(g.kind)) atomicMax(&dst[1], src[1]);
           else if (g.arg_et == 1) { for (int d = 0; d < F64_ACC_DIGITS; ++d) if (src[1 + d]) atomicAdd(&dst[1 + d], src[1 + d]); }
           else { atomicAdd(&dst[1], src[1]); atomicAdd(&dst[2], src[2]); }
         }

@@ -75,7 +75,7 @@ def f64_acc_value(words):
     return float(Fraction(total, 1 << 1074))
 
 
-def merge_agg_partials(keys, key_null, acc, real_words=(), max_words=()):
+def merge_agg_partials(keys, key_null, acc, real_words=(), max_words=(), word_ops=None, desc=False):
     """Final merge of partial aggregation tables.
 
     keys: int64[n] group-key bits, key_null: bool[n], acc: int64[n, W] additive accumulator words (b2_agg_partials).
@@ -84,10 +84,20 @@ def merge_agg_partials(keys, key_null, acc, real_words=(), max_words=()):
     `max_words` lists the word indices that merge by unsigned maximum (the MAX / MIN extremum keys,
     b2_agg_partials.max_word_mask); every other word is additive: counts, the 32-bit limb sums of integer SUMs and the
     digits of exact Real SUMs (`real_words` is only for callers that still carry plain f64 words).  Returns (keys, key_null, acc) with one row per group.
-    Integer words are summed exactly (two's-complement wraparound is impossible below 2^32 rows per group)."""
+    Integer words are summed exactly (two's-complement wraparound is impossible below 2^32 rows per group).
+    `word_ops` (agg_word_ops: one ffi.MERGE_* per word) adds the FIRST / BIT_* states: OR and XOR words reduce with their
+    op; a FIRST pair is taken from the earliest gathered part (rank order, the order of shard_blocks' contiguous runs)
+    holding a nonzero key, or the latest when the scan is `desc`; keys are compared only inside one part."""
+    from . import ffi
+    ops = list(word_ops) if word_ops is not None else []
+    max_words = set(max_words) | {w for w, o in enumerate(ops) if o == ffi.MERGE_MAX}
+    bit_words = {w: o for w, o in enumerate(ops) if o in (ffi.MERGE_OR, ffi.MERGE_XOR)}
+    first_words = [w for w, o in enumerate(ops) if o == ffi.MERGE_FIRST_KEY]
+    special = set(real_words) | max_words | set(bit_words) | {w for w, o in enumerate(ops) if o in (ffi.MERGE_FIRST_KEY, ffi.MERGE_FIRST_VALUE)}
     multi = keys.dim() == 2
     kw = keys.shape[1] if multi else 1
     parts = _all_gather_var(torch.cat([keys.view(-1, kw), key_null.to(torch.int64).view(-1, 1), acc], dim=1))
+    part_of = torch.cat([torch.full((p.shape[0],), i, dtype=torch.int64, device=p.device) for i, p in enumerate(parts)])
     allp = torch.cat(parts, dim=0)
     if allp.shape[0] == 0:
         return keys[:0], key_null[:0], acc[:0]
@@ -97,7 +107,29 @@ def merge_agg_partials(keys, key_null, acc, real_words=(), max_words=()):
     ident = torch.cat([nul.view(-1, 1), k], dim=1)
     uniq, inv = torch.unique(ident, dim=0, return_inverse=True)
     out = torch.zeros((uniq.shape[0], a.shape[1]), dtype=torch.int64, device=a.device)
-    int_words = [w for w in range(a.shape[1]) if w not in set(real_words) and w not in set(max_words)]
+    ng = uniq.shape[0]
+    for w, o in bit_words.items():  # per bit plane: OR = any row has it, XOR = an odd number of rows have it
+        for b0 in range(0, 64, 8):  # 8 one-byte planes at a time: 8 transient bytes per gathered row
+            shifts = torch.arange(b0, b0 + 8, device=a.device)
+            planes = ((a[:, w].view(-1, 1) >> shifts) & 1).to(torch.uint8)
+            red = torch.zeros((ng, 8), dtype=torch.uint8, device=a.device)
+            if o == ffi.MERGE_OR:
+                red.scatter_reduce_(0, inv.view(-1, 1).expand(-1, 8), planes, reduce="amax")
+            else:
+                red.index_add_(0, inv, planes)  # (a uint8 sum wraps mod 256 and keeps its parity)
+            out[:, w] |= ((red & 1).to(torch.int64) << shifts).sum(dim=1)  # (distinct bits: their sum is their OR)
+    for w in first_words:
+        has = a[:, w] != 0
+        pref = part_of if desc else len(parts) - 1 - part_of  # larger = preferred part
+        pref = torch.where(has, pref, torch.full_like(pref, -1))
+        best = torch.full((ng,), -1, dtype=torch.int64, device=a.device).scatter_reduce_(0, inv, pref, reduce="amax")
+        cand = has & (pref == best[inv])
+        flipped = torch.where(cand, a[:, w] ^ SIGN, torch.full_like(a[:, w], SIGN))  # unsigned order as signed
+        top = torch.full((ng,), SIGN, dtype=torch.int64, device=a.device).scatter_reduce_(0, inv, flipped, reduce="amax")
+        win = cand & (flipped == top[inv])
+        out[inv[win], w] = a[win, w]
+        out[inv[win], w + 1] = a[win, w + 1]
+    int_words = [w for w in range(a.shape[1]) if w not in special]
     if int_words:
         out[:, int_words] = torch.zeros((uniq.shape[0], len(int_words)), dtype=torch.int64, device=a.device).index_add_(0, inv, a[:, int_words])
     for w in real_words:
@@ -205,3 +237,18 @@ def agg_partials_as_tensors(executor, device):
         keys = torch.zeros(n, dtype=torch.int64, device=dev)
         nul = torch.zeros(n, dtype=torch.bool, device=dev)
     return keys, nul, acc
+
+
+def agg_word_ops(executor):
+    """How each accumulator word of the executor's partial table merges (b2_exec_agg_word_ops): a list of ffi.MERGE_*."""
+    import ctypes as C
+    from . import ffi
+    p = ffi.AggPartials()
+    rc = ffi.lib().b2_exec_agg_partials(executor._h, C.byref(p))
+    if rc == 0:
+        n = C.c_uint32(p.acc_words)
+        ops = (C.c_uint8 * max(1, p.acc_words))()
+        rc = ffi.lib().b2_exec_agg_word_ops(executor._h, ops, C.byref(n))
+    if rc != 0:
+        raise RuntimeError(ffi.lib().b2_last_error_message().decode())
+    return list(ops[: n.value])

@@ -35,6 +35,8 @@ def _header_enum(prefix):
 SIG = _header_enum("B2_SIG_")  # tipb::ScalarFuncSig numbers, never typed twice
 
 AGG_COUNT, AGG_SUM, AGG_AVG, AGG_MIN, AGG_MAX, AGG_FIRST = 3001, 3002, 3003, 3004, 3005, 3006
+AGG_BIT_AND, AGG_BIT_OR, AGG_BIT_XOR = 3008, 3009, 3010
+MERGE_ADD, MERGE_MAX, MERGE_OR, MERGE_XOR, MERGE_FIRST_KEY, MERGE_FIRST_VALUE = 0, 1, 2, 3, 4, 5  # b2_exec_agg_word_ops
 EXEC_TABLE_SCAN, EXEC_INDEX_SCAN, EXEC_SELECTION, EXEC_AGGREGATION, EXEC_TOPN, EXEC_LIMIT, EXEC_STREAM_AGG, EXEC_PROJECTION = range(8)
 COL_I64, COL_F64, COL_DECIMAL, COL_BYTES, COL_TIME, COL_DURATION, COL_JSON = 0, 1, 2, 3, 4, 5, 6
 DRAIN_REMAIN, DRAIN_DRAINED, DRAIN_PAGING = 0, 1, 2
@@ -175,7 +177,7 @@ JIT_AUTO, JIT_SYNC, JIT_OFF = 0, 1, 2
 EXPORTED_SYMBOLS = [
     "b2_abi_version", "b2_build_info", "b2_last_error_message", "b2_check_supported", "b2_plan_prepare", "b2_plan_precompile", "b2_jit_counters", "b2_plan_literal", "b2_exec_open", "b2_exec_schema",
     "b2_exec_next_batch", "b2_exec_next_batch_async", "b2_exec_poll", "b2_exec_warnings", "b2_region_pin", "b2_region_unpin", "b2_region_cache_stats", "b2_exec_collect_stats", "b2_exec_last_error", "b2_exec_can_be_cached", "b2_exec_encode_batch", "b2_exec_take_scanned_range", "b2_exec_collect_scanned_rows_per_range", "b2_exec_close",
-    "b2_exec_agg_partials", "b2_dag_handle", "b2_checksum_handle", "b2_gen_create", "b2_gen_destroy", "b2_copy_to_host", "b2_copy_to_device",
+    "b2_exec_agg_partials", "b2_exec_agg_word_ops", "b2_dag_handle", "b2_checksum_handle", "b2_gen_create", "b2_gen_destroy", "b2_copy_to_host", "b2_copy_to_device",
     "b2_sst_decode", "b2_sst_free", "b2_sst_encode",
     "b2_device_count", "b2_host_alloc_pinned", "b2_host_alloc_pinned_near", "b2_device_numa_node", "b2_host_free_pinned",
 ]
@@ -237,6 +239,8 @@ def lib():
     L.b2_exec_can_be_cached.restype = i32
     L.b2_exec_agg_partials.argtypes = [vp, C.POINTER(AggPartials)]
     L.b2_exec_agg_partials.restype = i32
+    L.b2_exec_agg_word_ops.argtypes = [vp, C.POINTER(C.c_uint8), C.POINTER(u32)]
+    L.b2_exec_agg_word_ops.restype = i32
     L.b2_exec_close.argtypes = [vp]
     L.b2_exec_close.restype = None
     L.b2_dag_handle.argtypes = [C.POINTER(DagPlan), C.POINTER(KeyRange), u32, C.POINTER(RegionSource), C.POINTER(ExecConfig), C.POINTER(Batch), C.POINTER(vp)]

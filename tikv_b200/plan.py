@@ -245,8 +245,9 @@ class Plan:
         return self
 
     def aggregation(self, aggs, group_by=()):
-        """aggs: list of (kind, Expr) with kind in {'count','sum','avg'}."""
-        kinds = {"count": ffi.AGG_COUNT, "sum": ffi.AGG_SUM, "avg": ffi.AGG_AVG, "min": ffi.AGG_MIN, "max": ffi.AGG_MAX}
+        """aggs: list of (kind, Expr) with kind in {'count','sum','avg','min','max','first','bit_and','bit_or','bit_xor'}."""
+        kinds = {"count": ffi.AGG_COUNT, "sum": ffi.AGG_SUM, "avg": ffi.AGG_AVG, "min": ffi.AGG_MIN, "max": ffi.AGG_MAX,
+                 "first": ffi.AGG_FIRST, "bit_and": ffi.AGG_BIT_AND, "bit_or": ffi.AGG_BIT_OR, "bit_xor": ffi.AGG_BIT_XOR}
         a = (ffi.AggrDesc * len(aggs))()
         for i, (k, ex) in enumerate(aggs):
             a[i].kind = kinds[k]
