@@ -174,11 +174,12 @@ def check_exact_real_sums(run, region):
     assert math.isclose(seq, math.fsum(allv), rel_tol=1e-12)  # the reference's sequential sum is only this close to it
 
 
-def topn_plans():
+def topn_plans(desc=False):
     """(name, Plan, exact) — exact=False when ties at the cut make the surviving rows ambiguous in the reference too
-    (TopNHeap keeps whichever tied rows its binary heap happens to hold): then only the sort keys are compared."""
+    (TopNHeap keeps whichever tied rows its binary heap happens to hold): then only the sort keys are compared.
+    desc=True: the same plans over a backward scan."""
     def scan():
-        return Plan().table_scan(TABLE, COLUMNS)
+        return Plan().table_scan(TABLE, COLUMNS, desc=desc)
     return [
         ("topn_two_keys", scan().topn([(col(C2), True), (col(C1), False)], 50).build(), True, None),
         ("topn_real_desc_handle", scan().topn([(col(C4, tp=ffi.TP_DOUBLE), True), (col(C_H), False)], 30).build(), True, None),

@@ -307,28 +307,28 @@ def test_topn_matches_oracle(name, plan, exact, keys, regions):
 
 
 def test_topn_large_generated():
-    """TopN over 3e6 generated rows in 3 blocks: ORDER BY c2 DESC, c1 ASC LIMIT 1000 (BASELINE config 4 shape)."""
+    """TopN over 3e6 generated rows in 3 blocks: ORDER BY c2 DESC, c1 ASC LIMIT 1000 (BASELINE config 4 shape), every
+    cell equal to the exact reference over the generator's closed form (topn_ref.py), on the whole table and on halves."""
+    import topn_ref
     n_rows, n_cols, seed = 3_000_000, 4, 99
-    gens, blocks, hosts, keep = [], [], [], []
-    for i in range(3):
-        g, blk = _gen_block(n_rows // 3, n_cols, 2, seed, [0, 0, 0, 0], [0, 0, 0, 0], [0, 10000, 0, 0], first_handle=i * (n_rows // 3))
+    spec = dict(n_cols=n_cols, seed=seed, lo=[0] * 4, rng=[0] * 4, nulls=[0, 10000, 0, 0])
+    parts = [(i * (n_rows // 3), n_rows // 3) for i in range(3)]
+    gens, blocks = [], []
+    for first, n in parts:
+        g, blk = _gen_block(n, n_cols, 2, seed, spec["lo"], spec["rng"], spec["nulls"], first_handle=first)
         gens.append(g); blocks.append(blk.block)
     try:
         dev = _source(blocks, ffi.LOC_DEVICE)
         columns = [ColumnDef(100, pk_handle=True)] + [ColumnDef(i + 1) for i in range(n_cols)]
         plan = Plan().table_scan(sc.TABLE, columns).topn([(col(2), True), (col(1), False)], 1000).build()
-        got = DagHandler(plan, sc.WHOLE, dev).handle_request()
-        assert got.status == 0 and got.n_rows == 1000
-        rows = got.rows()
-        # sortedness under (c2 DESC with NULL last, c1 ASC), and every returned row beats a sampled non-returned one
-        def key(r):
-            return (1 if r[2] is None else 0, -(r[2] or 0), r[1])
-        assert rows == sorted(rows, key=key)
-        # idempotence / partition property: top-N of the union == top-N of (top-N of each part)
-        parts = []
-        for lo, hi in ((0, n_rows // 2), (n_rows // 2, n_rows)):
-            parts += DagHandler(plan, [kvfmt.table_range(sc.TABLE, lo, hi)], dev).handle_request().rows()
-        assert sorted(parts, key=key)[:1000] == rows
+        ref = topn_ref.gen_rows(spec, parts)
+        h, v, nl = ref["handle"], ref["vals"], ref["null"]
+        for lo, hi in ((0, n_rows), (0, n_rows // 2), (n_rows // 2, n_rows)):
+            idx = np.flatnonzero((h >= lo) & (h < hi))
+            best = idx[topn_ref.topn_indices([(v[idx, 1], nl[idx, 1], True), (v[idx, 0], nl[idx, 0], False)], 1000)]
+            want = [(int(h[i]),) + tuple(None if nl[i, c] else int(v[i, c]) for c in range(n_cols)) for i in best]
+            got = DagHandler(plan, [kvfmt.table_range(sc.TABLE, lo, hi)], dev).handle_request()
+            assert got.status == 0 and got.rows() == want, (lo, hi)
     finally:
         for g in gens:
             ffi.lib().b2_gen_destroy(g)

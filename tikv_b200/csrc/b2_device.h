@@ -141,7 +141,11 @@ struct DevPlan {
   uint64_t limit;
   DevExpr conds[MAX_CONDS];
   DevExpr group;
-  uint8_t group_et, group_unsigned, _p0, _p1;
+  uint8_t group_et, group_unsigned;
+  uint8_t topn_all_keys;       // PM_TOPN: 1 = a sort key after the first can fail or warn (it is not a plain column or constant):
+                               //   the lean kernel evaluates every sort key of every row, as the reference does, instead of
+                               //   only those of the rows whose first key can still beat the CTA's bound
+  uint8_t _p1;
   DevAgg aggs[MAX_AGGS];
   DevOrder order[MAX_ORDER];
   uint8_t out_cols[MAX_COLS];
@@ -2240,13 +2244,14 @@ B2_HD bool first_key_may_beat(const DevPlan& P, const Value& v0, const TopItem& 
   return c <= 0;
 }
 
-B2_HD int make_item(const DevPlan& P, const Row& row, const Cells& cells, uint64_t id, TopItem* it) {
+// `first`: the row's first sort key when the caller has evaluated it already (evaluated twice, it would warn twice)
+B2_HD int make_item(const DevPlan& P, const Row& row, const Cells& cells, uint64_t id, TopItem* it, const Value* first = nullptr) {
   it->nulls = 0; it->id = id; it->slot = 0;
   for (int k = 0; k < MAX_ORDER; ++k) it->w[k] = 0;
   for (int k = 0; k < P.n_order; ++k) {
     Value v;
-    int e = eval_expr(P, P.order[k].e, row, cells, &v, nullptr);
-    if (e) return e;
+    if (k == 0 && first) v = *first;
+    else if (int e = eval_expr(P, P.order[k].e, row, cells, &v, nullptr)) return e;
     if (v.null) { it->nulls |= 1u << k; continue; }
     it->w[k] = order_key_word(P.order[k], v.bits);
   }

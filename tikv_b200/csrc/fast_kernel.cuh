@@ -236,11 +236,12 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
               if (a < P.n_aggs && ok) ok = eval_expr(P, P.aggs[a].arg, row, cells, &av[a], nullptr) == 0;
           } else {
             // most rows lose against the CTA's threshold on their first sort key alone (the threshold only changes inside a
-            // CTA-wide compaction, so reading it here is race-free)
+            // CTA-wide compaction, so reading it here is race-free).  When a later key can fail or warn, every row evaluates
+            // all of them: a request's error and warning count must not depend on which rows the bound let through.
             Value v0;
             ok = eval_expr(P, P.order[0].e, row, cells, &v0, nullptr) == 0;
-            cand = ok && (!s_top_have_thr || first_key_may_beat(P, v0, s_top_thr));
-            if (cand) ok = make_item(P, row, cells, A.desc ? ~(A.entry_base + e) : A.entry_base + e, &item) == 0;
+            cand = ok && (P.topn_all_keys || !s_top_have_thr || first_key_may_beat(P, v0, s_top_thr));
+            if (cand) ok = make_item(P, row, cells, A.desc ? ~(A.entry_base + e) : A.entry_base + e, &item, &v0) == 0;
           }
         }
         if (!ok) { push = true; commit = false; }  // the general decoder / evaluator owns this run (and raises its error)

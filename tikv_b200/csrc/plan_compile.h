@@ -462,6 +462,8 @@ inline int compile_plan(const b2_dag_plan* plan, CompiledPlan* out, std::string*
         uint8_t et, uns;
         if (!lower_expr(e.order_by[k].expr, P, &o.e, &et, &uns, nullptr, nullptr, msg)) return B2_ERR_UNSUPPORTED;
         o.desc = e.order_by[k].desc ? 1 : 0; o.et = et; o.is_unsigned = uns;
+        const DevNode& root = P.nodes[o.e.start + o.e.n - 1];
+        if (k > 0 && (o.e.n != 1 || root.kind == B2_RPN_FN)) P.topn_all_keys = 1;  // (a column or a constant cannot fail or warn)
       }
       if (e.limit > 2048) { *msg = "TopN limit above 2048 is not on the device path yet"; return B2_ERR_UNSUPPORTED; }
       P.n_order = (int)e.n_order_by; P.limit = e.limit;

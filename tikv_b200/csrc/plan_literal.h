@@ -22,7 +22,7 @@ inline std::string plan_literal(const DevPlan& P) {
   u64(P.fast_ids); o << ","; u64(0 /* read_ts stays a launch parameter */); o << ","; u64(0 /* so does the TopN limit (ScanArgs::limit) */); o << ",{";
   for (int i = 0; i < MAX_CONDS; ++i) { expr(P.conds[i]); o << (i < MAX_CONDS - 1 ? "," : ""); }
   o << "},"; expr(P.group);
-  o << "," << (int)P.group_et << "," << (int)P.group_unsigned << "," << (int)P._p0 << "," << (int)P._p1 << ",{";
+  o << "," << (int)P.group_et << "," << (int)P.group_unsigned << "," << (int)P.topn_all_keys << "," << (int)P._p1 << ",{";
   for (int i = 0; i < MAX_AGGS; ++i) {
     const DevAgg& a = P.aggs[i];
     o << "{"; expr(a.arg); o << "," << (int)a.kind << "," << (int)a.arg_et << "," << (int)a.arg_unsigned << "," << (int)a.acc_off << "}" << (i < MAX_AGGS - 1 ? "," : "");
