@@ -261,7 +261,7 @@ typedef struct b2_executor_desc {
   const b2_order_by* order_by;        /* TopN */
   uint32_t n_order_by;
   uint32_t _pad;
-  uint64_t limit;                     /* TopN / Limit */
+  uint64_t limit;                     /* TopN (at most 4096 on the device path) / Limit */
 } b2_executor_desc;
 
 typedef struct b2_dag_plan {

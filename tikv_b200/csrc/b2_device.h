@@ -37,7 +37,8 @@ namespace b2 {
 
 // ---- limits of the device plan ----
 enum { MAX_GROUP = 4, MAX_PROJ = 16, MAX_COLS = 64, MAX_NODES = 96, MAX_CONDS = 8, MAX_AGGS = 8, MAX_ORDER = 4, MAX_STACK = 16, MAX_ACC_WORDS = 144,
-       MAX_IMMS = 48 /* constants of a plan that travel as launch parameters instead of being part of the (compiled) plan */ };
+       MAX_IMMS = 48 /* constants of a plan that travel as launch parameters instead of being part of the (compiled) plan */,
+       MAX_TOPN_LIMIT = 4096 /* per-CTA candidate lists cost CTAs x limit x sizeof(TopItem) of HBM (engine.cu run_topn) */ };
 
 // ---- device error codes (mapped to B2_ERR_* + message in engine.cu) ----
 enum DevErr {

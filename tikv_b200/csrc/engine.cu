@@ -403,6 +403,19 @@ struct b2_exec {
     if (const JitKernel* k = jit_ready()) { stats.jit_launches++; return jit_launch(k, a, grid, smem, stream); }
     return launch_scan(cp.dev, a, grid, smem, stream);
   }
+  // The general kernel of an order-free launch.  A TopN whose candidate buffers are in HBM (a.topn_work set: LIMIT above
+  // 2048) runs its own instantiation (plan-specialised b2_scan_topn_hbm_jit, or the generic scan_topn_hbm_kernel), so
+  // the shared-memory TopN kernels keep their code.
+  int topn_hbm_grid(size_t smem) {
+    if (const JitKernel* k = jit_ready()) return jit_max_blocks_per_sm(k, smem, JIT_TOPN_HBM) * scan_num_sms();
+    return scan_topn_hbm_max_grid(smem);
+  }
+  int general_grid_for(const ScanArgs& a, int mode, size_t smem) { return mode == PM_TOPN && a.topn_work ? topn_hbm_grid(smem) : scan_grid_for(mode, smem); }
+  cudaError_t general_launch(const ScanArgs& a, int mode, int grid, size_t smem) {
+    if (!(mode == PM_TOPN && a.topn_work)) return scan_launch(a, grid, smem);
+    if (const JitKernel* k = jit_ready()) { stats.jit_launches++; return jit_launch(k, a, grid, smem, stream, JIT_TOPN_HBM); }
+    return launch_scan_topn_hbm(cp.dev, a, grid, smem, stream);
+  }
 
   // Row format of the first row a unit will touch (TiDB tables are all-v1 or all-v2 in practice); decides whether the
   // v1 twin of the exact-layout path is part of the kernel.  A wrong guess only costs speed: every row is checked.
@@ -815,17 +828,19 @@ struct b2_exec {
   DevBuf const_pool;  // bytes constants of the plan (CompiledPlan::pool)
   bool fast_kernel_covers() const { return cp.dev.mode == PM_CHECKSUM || plan_has_fast_kernel(cp.dev); }
   // `a`: the unit's arguments (c_lo / c_hi set, mode pointers set).  general_smem_mode / fast_smem_mode: bytes of mode state
-  // in front of the stages; fast_slots: CTA table slots of the lean aggregation kernel.
+  // in front of the stages; fast_slots: CTA table slots of the lean aggregation kernel.  TopN: a0.topn_work is the lean
+  // kernel's candidate area, and the general kernel's too when general_smem_mode is 0 (the launches are stream-ordered).
   int launch_unit(const ScanArgs& a0, const Unit& u, bool fast, size_t general_smem_mode, size_t fast_smem_mode, uint32_t fast_slots, int* general_grid_out,
                   int* fast_grid_out) {
     const int mode = scan_kernel_mode(cp.dev);
     if (!fast) {
       ScanArgs a = a0;
+      if (general_smem_mode) a.topn_work = nullptr;
       size_t tot = setup_staging(&a, wblocks[u.block_idx], general_smem_mode);
-      int grid = scan_grid_for(mode, tot);
+      int grid = general_grid_for(a, mode, tot);
       if (general_grid_out && *general_grid_out > 0) grid = std::min(grid, *general_grid_out);
       kernel_begin();
-      CUDA_TRY(scan_launch(a, grid, tot));
+      CUDA_TRY(general_launch(a, mode, grid, tot));
       kernel_end();
       if (general_grid_out) *general_grid_out = grid;
       if (fast_grid_out) *fast_grid_out = 0;
@@ -840,16 +855,17 @@ struct b2_exec {
     size_t ftot = setup_staging(&f, wblocks[u.block_idx], fast_smem_mode);
     const JitKernel* jk = jit_ready();
     if (jk && !jk->fn_fast) jk = nullptr;
-    int fgrid = jk ? jit_max_blocks_per_sm(jk, ftot, true) * scan_num_sms() : fast_max_grid(cp.dev.mode, ftot);
+    int fgrid = jk ? jit_max_blocks_per_sm(jk, ftot, JIT_FAST) * scan_num_sms() : fast_max_grid(cp.dev.mode, ftot);
     if (fast_grid_out && *fast_grid_out > 0) fgrid = std::min(fgrid, *fast_grid_out);
     kernel_begin();
     if (f.staging) {
-      if (jk) { stats.jit_launches++; CUDA_TRY(jit_launch(jk, f, fgrid, ftot, stream, true)); }
+      if (jk) { stats.jit_launches++; CUDA_TRY(jit_launch(jk, f, fgrid, ftot, stream, JIT_FAST)); }
       else CUDA_TRY(launch_fast(cp.dev, f, fgrid, ftot, stream));
     } else {  // no staging possible (huge entries): everything goes through the general kernel
       fast = false;
     }
     ScanArgs g = a0;
+    if (general_smem_mode) g.topn_work = nullptr;
     size_t gtot = general_smem_mode;
     if (fast) {
       g.slow_list = f.slow_list; g.slow_count = f.slow_count; g.list_mode = 1;
@@ -857,12 +873,12 @@ struct b2_exec {
     } else {
       gtot = setup_staging(&g, wblocks[u.block_idx], general_smem_mode);
     }
-    int ggrid = scan_grid_for(mode, gtot);
+    int ggrid = general_grid_for(g, mode, gtot);
     if (general_grid_out && *general_grid_out > 0) ggrid = std::min(ggrid, *general_grid_out);
     if (cp.dev.mode == PM_TOPN && fast) {  // the two kernels leave their per-CTA lists side by side
       g.topn.items = a0.topn.items + (size_t)fgrid * a0.topn.stride; g.topn.counts = a0.topn.counts + fgrid;
     }
-    CUDA_TRY(scan_launch(g, ggrid, gtot));
+    CUDA_TRY(general_launch(g, mode, ggrid, gtot));
     kernel_end();
     stats.kernel_launches += fast ? 1 : 0;
     if (general_grid_out) *general_grid_out = ggrid;
@@ -1574,21 +1590,30 @@ struct b2_exec {
     if (rc) return rc;
     uint32_t n = 0;
     if (limit > 0 && !units.empty()) {  // top_n_executor.rs:304-312: n == 0 drains immediately
+      // Up to LIMIT 2048 the general kernel keeps its candidate buffer in shared memory, `cap` a power of two >= limit + TILE.
+      // Above that the buffer would not fit next to the TMA stages, so both kernels keep theirs in HBM, and cap = 8192
+      // (a power of two >= 2 x limit): a CTA compacts after at least cap - limit - 2 x TILE new candidates (3584 at
+      // LIMIT 4096), where cap = limit + TILE rounded up would compact at almost every rendezvous.
+      const bool big = limit > 2048;
       uint32_t cap = 512;
-      while (cap < limit + TILE) cap <<= 1;
-      size_t smem = topn_smem_bytes(cap, P.n_order);
+      while (cap < (big ? 2 * limit : limit + TILE)) cap <<= 1;
+      const size_t buf_bytes = topn_smem_bytes(cap, P.n_order);  // one CTA's candidate buffer
+      const size_t smem = big ? 0 : buf_bytes;                     // the general kernel's mode bytes in shared memory
       ScanArgs probe; memset(&probe, 0, sizeof(probe));
       size_t tot0 = setup_staging(&probe, wblocks[units[0].block_idx], smem);
-      int grid = scan_grid_for(PM_TOPN, std::max(tot0, smem));
+      int grid = big ? topn_hbm_grid(tot0) : scan_grid_for(PM_TOPN, std::max(tot0, smem));
       const bool any_fast = fast_kernel_covers();
       int fast_grid = 0;
       if (any_fast) {  // the lean kernel keeps its candidate buffers in HBM (ScanArgs::topn_work): shared memory holds the stages only
         const JitKernel* jk = jit_ready();
         ScanArgs fprobe; memset(&fprobe, 0, sizeof(fprobe));
         const size_t ftot0 = setup_staging(&fprobe, wblocks[units[0].block_idx], 0);
-        fast_grid = jk && jk->fn_fast ? jit_max_blocks_per_sm(jk, ftot0, true) * scan_num_sms() : fast_max_grid(PM_TOPN, ftot0);
-        CUDA_TRY(tn_work.reserve((size_t)fast_grid * smem));
+        fast_grid = jk && jk->fn_fast ? jit_max_blocks_per_sm(jk, ftot0, JIT_FAST) * scan_num_sms() : fast_max_grid(PM_TOPN, ftot0);
       }
+      // the lean launch of a chunk and the general one behind it run one after the other on the stream: above LIMIT 2048
+      // they share one work area, sized for the larger grid
+      const int work_ctas = big ? std::max(grid, fast_grid) : fast_grid;
+      if (work_ctas) CUDA_TRY(tn_work.reserve((size_t)work_ctas * buf_bytes));
       const int lists_cap = grid + fast_grid;  // the lean and the general kernel leave their per-CTA lists side by side
       size_t isz = sizeof(TopItem);
       CUDA_TRY(tn_lists.reserve((size_t)lists_cap * limit * isz)); CUDA_TRY(tn_counts.reserve((size_t)lists_cap * 4));
@@ -1628,7 +1653,7 @@ struct b2_exec {
         a.topn.items = (TopItem*)tn_lists.p; a.topn.counts = (unsigned int*)tn_counts.p; a.topn.stride = limit;
         a.topn_cap = cap;
         a.topn_seed = run_items; a.topn_seed_cnt = run_cnt;
-        a.topn_work = (unsigned char*)tn_work.p; a.topn_work_stride = smem;
+        a.topn_work = (unsigned char*)tn_work.p; a.topn_work_stride = buf_bytes;
         CUDA_TRY(cudaMemsetAsync(tn_counts.p, 0, (size_t)lists_cap * 4, stream));
         const bool fast = any_fast && u.fast_ok;
         int gg = (int)std::min<uint32_t>((uint32_t)grid, n_tiles), fg = (int)std::min<uint32_t>((uint32_t)std::max(fast_grid, 1), n_tiles);

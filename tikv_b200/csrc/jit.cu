@@ -151,7 +151,7 @@ JitSpec jit_spec(const DevPlan& plan) {
 // holding the full key (a hash collision or a stale file is detected by comparing it).  Written atomically (rename).
 std::atomic<unsigned long long> g_nvrtc_compiles{0}, g_cache_hits{0};
 std::string cache_key(const JitSpec& j) {
-  return "b2jit5|sm_90a|mode" + std::to_string(j.mode) + "|ext" + std::to_string((int)j.ext_sigs) + "|fast" + std::to_string(j.fast) + "|src" + std::to_string(api().src_hash) + "|" + j.literal;
+  return "b2jit6|sm_90a|mode" + std::to_string(j.mode) + "|ext" + std::to_string((int)j.ext_sigs) + "|fast" + std::to_string(j.fast) + "|src" + std::to_string(api().src_hash) + "|" + j.literal;
 }
 std::string cache_path(const std::string& key, const std::string& dir = api().cache_dir) {
   char name[32];
@@ -196,6 +196,9 @@ bool compile_cubin(const JitSpec& j, std::vector<char>* cubin, std::string* erro
   if (j.fast & 1)
     src += "extern \"C\" __global__ void __launch_bounds__(b2::FK_THREADS, 3) b2_fast_jit(const __grid_constant__ b2::ScanArgs A) {\n"
            "  b2::fast_body<" + std::to_string(j.mode) + ">(b2::kJitPlan, A);\n}\n";
+  if (j.mode == PM_TOPN)  // the limit is a launch parameter: every TopN module also carries the large-limit variant
+    src += "extern \"C\" __global__ void __launch_bounds__(b2::TILE + 64, 2) b2_scan_topn_hbm_jit(const __grid_constant__ b2::ScanArgs A) {\n"
+           "  b2::scan_body<" + std::to_string(j.mode) + ", true>(b2::kJitPlan, A);\n}\n";
   nvrtcProgram prog;
   if (a.CreateProgram(&prog, src.c_str(), "b2_scan_jit.cu", 0, nullptr, nullptr) != NVRTC_SUCCESS) { *error = "nvrtcCreateProgram failed"; return false; }
   std::string inc = "-I" + a.csrc_dir;
@@ -241,6 +244,11 @@ JitKernel* compile(int device, const JitSpec& j) {
     CUfunction ff;
     if (a.ModuleGetFunction(&ff, mod, "b2_fast_jit") != CUDA_SUCCESS) { k->error = "lean kernel symbol missing"; return k; }
     k->fn_fast = ff;
+  }
+  if (j.mode == PM_TOPN) {
+    CUfunction fh;
+    if (a.ModuleGetFunction(&fh, mod, "b2_scan_topn_hbm_jit") != CUDA_SUCCESS) { k->error = "large-limit TopN kernel symbol missing"; return k; }
+    k->fn_topn_hbm = fh;
   }
   k->ok = true;
   return k;
@@ -302,10 +310,14 @@ int jit_precompile(const DevPlan& plan, std::string* error) {
 }
 void jit_counters(unsigned long long* nvrtc_compiles, unsigned long long* disk_hits) { *nvrtc_compiles = g_nvrtc_compiles.load(); *disk_hits = g_cache_hits.load(); }
 
-int jit_max_blocks_per_sm(const JitKernel* k, size_t smem, bool fast) {
+static CUfunction entry_fn(const JitKernel* k, JitEntry e) { return (CUfunction)(e == JIT_FAST ? k->fn_fast : e == JIT_TOPN_HBM ? k->fn_topn_hbm : k->fn); }
+static size_t& entry_smem(const JitKernel* k, JitEntry e) { return e == JIT_FAST ? k->max_dyn_smem_fast : e == JIT_TOPN_HBM ? k->max_dyn_smem_topn_hbm : k->max_dyn_smem; }
+
+int jit_max_blocks_per_sm(const JitKernel* k, size_t smem, JitEntry entry) {
   int n = 0;
-  CUfunction fn = (CUfunction)(fast ? k->fn_fast : k->fn);
-  size_t& lim = fast ? k->max_dyn_smem_fast : k->max_dyn_smem;
+  const bool fast = entry == JIT_FAST;
+  CUfunction fn = entry_fn(k, entry);
+  size_t& lim = entry_smem(k, entry);
   if (smem > lim) {
     std::lock_guard<std::mutex> lk(g_mu);
     if (smem > lim && api().FuncSetAttribute(fn, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem) == CUDA_SUCCESS) lim = smem;
@@ -314,13 +326,14 @@ int jit_max_blocks_per_sm(const JitKernel* k, size_t smem, bool fast) {
   return n;
 }
 
-cudaError_t jit_launch(const JitKernel* k, const ScanArgs& a, int grid, size_t smem, cudaStream_t s, bool fast) {
+cudaError_t jit_launch(const JitKernel* k, const ScanArgs& a, int grid, size_t smem, cudaStream_t s, JitEntry entry) {
   if (a.c_hi <= a.c_lo) return cudaSuccess;
   uint32_t n_tiles = (a.c_hi - a.c_lo + TILE - 1) / TILE;
   if ((uint32_t)grid > n_tiles) grid = (int)n_tiles;
   void* params[] = {const_cast<ScanArgs*>(&a)};
-  CUfunction fn = (CUfunction)(fast ? k->fn_fast : k->fn);
-  size_t& lim = fast ? k->max_dyn_smem_fast : k->max_dyn_smem;
+  const bool fast = entry == JIT_FAST;
+  CUfunction fn = entry_fn(k, entry);
+  size_t& lim = entry_smem(k, entry);
   if (smem > lim) {  // opt in to large dynamic shared memory (the limit excludes the kernel's static part)
     std::lock_guard<std::mutex> lk(g_mu);
     if (smem > lim) {

@@ -7,7 +7,8 @@
 //                         flushed into the HBM group table (BatchSimpleAggregation / BatchFastHashAggregation)
 //   scan_kernel<PM_AGGM>  GROUP BY over 2..4 expressions: composite keys in a hash-tagged HBM table
 //                         (BatchSlowHashAggregation; slow_hash_aggr_executor.rs)
-//   scan_kernel<PM_TOPN>  per-CTA candidate buffers + threshold, merged by topn_rank_merge / gathered by topn_gather (BatchTopN)
+//   scan_kernel<PM_TOPN>  per-CTA candidate buffers + threshold, merged by topn_rank_merge / gathered by topn_gather (BatchTopN);
+//                         scan_topn_hbm_kernel: the same with the buffers in HBM (LIMIT above 2048)
 //   scan_kernel<PM_CHECKSUM>  CRC-64/XZ per KV, XOR-folded (checksum.rs)
 //   agg_finalize / agg_result, topn_*, pack_nulls, bounds: result materialisation; gen_*: synthetic region generator (tooling)
 // The same device body (scan_kernel.cuh) is compiled per plan at run time by jit.cu.
@@ -28,6 +29,11 @@ __global__ void __launch_bounds__(FK_THREADS, 2) fast_kernel(const __grid_consta
 template <int MODE>
 __global__ void __launch_bounds__(TILE + 64, 2) scan_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ ScanArgs A) {
   scan_body<MODE>(P, A);
+}
+
+// PM_TOPN above LIMIT 2048: the same body with the candidate buffer in HBM (one generic kernel serves every plan)
+__global__ void __launch_bounds__(TILE + 64, 2) scan_topn_hbm_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ ScanArgs A) {
+  scan_body<PM_TOPN, true>(P, A);
 }
 
 static int g_num_sms = 0;
@@ -92,6 +98,21 @@ cudaError_t launch_scan(const DevPlan& plan, const ScanArgs& a, int grid, size_t
     case PM_AGGM: scan_launch_mode<PM_AGGM>(plan, a, grid, smem, s); break;
     default: scan_launch_mode<PM_AGG>(plan, a, grid, smem, s); break;
   }
+  return cudaGetLastError();
+}
+
+int scan_topn_hbm_max_grid(size_t smem) {
+  int per_sm = 0;
+  if (smem > 48 * 1024) cudaFuncSetAttribute(scan_topn_hbm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, scan_topn_hbm_kernel, TILE + 64, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+  return per_sm * num_sms();
+}
+cudaError_t launch_scan_topn_hbm(const DevPlan& plan, const ScanArgs& a, int grid, size_t smem, cudaStream_t s) {
+  if (a.c_hi <= a.c_lo) return cudaSuccess;
+  const uint32_t n_tiles = (a.c_hi - a.c_lo + TILE - 1) / TILE;
+  if ((uint32_t)grid > n_tiles) grid = (int)n_tiles;
+  if (smem > 48 * 1024) cudaFuncSetAttribute(scan_topn_hbm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  scan_topn_hbm_kernel<<<grid, TILE + 64, smem, s>>>(plan, a);
   return cudaGetLastError();
 }
 

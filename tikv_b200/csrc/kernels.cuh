@@ -99,11 +99,12 @@ struct ScanArgs {
   uint8_t ck_new_prefix[32];
   // PM_TOPN
   TopNLists topn;                   // per-CTA result lists (stride = limit)
-  uint32_t topn_cap;                // shared-memory candidate capacity (power of two >= limit + TILE)
+  uint32_t topn_cap;                // candidate capacity of a CTA (engine.cu run_topn: power of two >= limit + TILE, 8192 above LIMIT 2048)
   const TopItem* topn_seed;         // running top-N of the units already merged (sorted), or nullptr:
   const unsigned int* topn_seed_cnt;  //   once it holds `limit` rows its last one is every CTA's initial threshold
   unsigned char* topn_work;           // lean TopN kernel: the CTAs' candidate buffers live in HBM / L2 (topn_work + blockIdx.x * stride): a
-  unsigned long long topn_work_stride;//   seeded CTA touches its buffer for a handful of rows per launch, and shared memory buys a third CTA per SM
+  unsigned long long topn_work_stride;//   seeded CTA touches its buffer for a handful of rows per launch, and shared memory buys a third CTA per SM.
+                                      //   Above LIMIT 2048 the general kernel's buffers live there too (scan_topn_hbm_kernel)
 };
 
 struct GenArgs {
@@ -122,6 +123,9 @@ int fast_max_grid(int mode, size_t smem);
 size_t fast_stage_bytes(uint32_t key_cap, uint32_t val_cap);
 size_t fast_checksum_bytes();             // PM_CHECKSUM tables + per-length key states
 int scan_max_grid(int mode, size_t smem);  // occupancy-based persistent grid size
+// the general TopN kernel with its candidate buffers in HBM (a.topn_work; LIMIT above 2048): grid size, launch
+int scan_topn_hbm_max_grid(size_t smem);
+cudaError_t launch_scan_topn_hbm(const DevPlan& plan, const ScanArgs& a, int grid, size_t smem, cudaStream_t s);
 int scan_num_sms();
 size_t scan_stage_bytes(uint32_t key_cap, uint32_t val_cap);  // dynamic shared memory needed by the tile stages
 size_t scan_crc_table_bytes();             // PM_CHECKSUM replicated CRC table

@@ -465,7 +465,7 @@ inline int compile_plan(const b2_dag_plan* plan, CompiledPlan* out, std::string*
         const DevNode& root = P.nodes[o.e.start + o.e.n - 1];
         if (k > 0 && (o.e.n != 1 || root.kind == B2_RPN_FN)) P.topn_all_keys = 1;  // (a column or a constant cannot fail or warn)
       }
-      if (e.limit > 2048) { *msg = "TopN limit above 2048 is not on the device path yet"; return B2_ERR_UNSUPPORTED; }
+      if (e.limit > MAX_TOPN_LIMIT) { *msg = "TopN limit above 4096 is not on the device path"; return B2_ERR_UNSUPPORTED; }
       P.n_order = (int)e.n_order_by; P.limit = e.limit;
     } else if (e.tp == B2_EXEC_PROJECTION) {
       if (P.mode != PM_SCAN || P.n_proj) { *msg = "Projection is on the device path only on top of a scan / selection pipeline"; return B2_ERR_UNSUPPORTED; }

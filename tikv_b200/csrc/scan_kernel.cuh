@@ -418,7 +418,10 @@ struct SmemTable {  // per-CTA group table (dynamic shared memory): keys | acc. 
 
 // The whole kernel as a device function: instantiated by the generic __global__ wrapper (plan in a __grid_constant__
 // parameter) and by the per-plan JIT translation unit (plan as a compile-time constant, jit.cpp).
-template <int MODE>
+// TOPN_HBM (PM_TOPN only): the CTA's candidate buffer is in HBM (ScanArgs::topn_work) instead of dynamic shared memory,
+// for LIMIT above 2048.  A template flag rather than a run-time choice: the shared-memory kernels keep their constant
+// shared-window addresses, and with them their registers and spills.
+template <int MODE, bool TOPN_HBM = false>
 __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
   // PM_PROJ is PM_SCAN with expression-valued output cells: a separate instantiation, so that the expression evaluator
   // stays out of the plain scan's hot loop (inlined there it cost 3.5x)
@@ -450,10 +453,10 @@ __device__ __forceinline__ void scan_body(const DevPlan& P, const ScanArgs& A) {
     __syncthreads();
   }
 
-  // PM_TOPN: per-CTA candidate buffer (dynamic shared memory) + current threshold
+  // PM_TOPN: per-CTA candidate buffer (dynamic shared memory, or HBM: topn_work + blockIdx.x * stride) + current threshold
   __shared__ unsigned int s_top_cnt, s_top_have_thr;
   __shared__ TopItem s_top_thr;
-  const TopBuf tb = topbuf_make(dyn_smem, MODE == PM_TOPN ? A.topn_cap : 0u, P);
+  const TopBuf tb = topbuf_make(TOPN_HBM ? A.topn_work + (size_t)blockIdx.x * A.topn_work_stride : dyn_smem, MODE == PM_TOPN ? A.topn_cap : 0u, P);
   if (MODE == PM_TOPN) {
     if (tid == 0) {
       s_top_cnt = 0; s_top_have_thr = 0;
