@@ -824,65 +824,172 @@ struct b2_exec {
   }
   // ---- order-free pipelines: the lean kernel (fast_kernel.cuh) over a unit, then scan_body in list mode over the runs it
   // handed over (their first entries, appended on the device; the count never visits the host) ----
-  DevBuf slow_list, slow_cnt;
+  DevBuf slow_list;
   DevBuf const_pool;  // bytes constants of the plan (CompiledPlan::pool)
   bool fast_kernel_covers() const { return cp.dev.mode == PM_CHECKSUM || plan_has_fast_kernel(cp.dev); }
-  // `a`: the unit's arguments (c_lo / c_hi set, mode pointers set).  general_smem_mode / fast_smem_mode: bytes of mode state
-  // in front of the stages; fast_slots: CTA table slots of the lean aggregation kernel.  TopN: a0.topn_work is the lean
-  // kernel's candidate area, and the general kernel's too when general_smem_mode is 0 (the launches are stream-ordered).
-  int launch_unit(const ScanArgs& a0, const Unit& u, bool fast, size_t general_smem_mode, size_t fast_smem_mode, uint32_t fast_slots, int* general_grid_out,
-                  int* fast_grid_out) {
+  // The general kernel over one unit.  `a`: the unit's arguments (c_lo / c_hi set, mode pointers set); general_smem_mode:
+  // bytes of mode state in front of the stages.  TopN: a.topn_work is the general kernel's candidate area when
+  // general_smem_mode is 0.
+  int launch_general(const ScanArgs& a0, uint32_t block_idx, size_t general_smem_mode, int* general_grid_out) {
+    ScanArgs a = a0;
+    if (general_smem_mode) a.topn_work = nullptr;
+    size_t tot = setup_staging(&a, wblocks[block_idx], general_smem_mode);
     const int mode = scan_kernel_mode(cp.dev);
-    if (!fast) {
-      ScanArgs a = a0;
-      if (general_smem_mode) a.topn_work = nullptr;
-      size_t tot = setup_staging(&a, wblocks[u.block_idx], general_smem_mode);
-      int grid = general_grid_for(a, mode, tot);
-      if (general_grid_out && *general_grid_out > 0) grid = std::min(grid, *general_grid_out);
-      kernel_begin();
-      CUDA_TRY(general_launch(a, mode, grid, tot));
-      kernel_end();
-      if (general_grid_out) *general_grid_out = grid;
-      if (fast_grid_out) *fast_grid_out = 0;
-      return B2_OK;
+    int grid = general_grid_for(a, mode, tot);
+    if (general_grid_out && *general_grid_out > 0) grid = std::min(grid, *general_grid_out);
+    kernel_begin();
+    CUDA_TRY(general_launch(a, mode, grid, tot));
+    kernel_end();
+    if (general_grid_out) *general_grid_out = grid;
+    return B2_OK;
+  }
+
+  // ---- lean launch groups: the lean kernel walks a table of units (UnitDesc) in one launch.  The descriptors of a
+  // request live in pinned memory (h_units, filled by the caller) and in HBM (units_dev, uploaded by upload_units); per
+  // descriptor there is a tile counter and a hand-over count (unit_ctrs: n tile counters, then n counts), zeroed once per
+  // request (reset_units).  A descriptor's pinned copy is written once before the request waits for its stream. ----
+  DevBuf units_dev, unit_ctrs;
+  HostBuf h_units;
+  std::vector<uint32_t> desc_block;  // the CF_WRITE block of each descriptor
+  size_t n_desc = 0;
+  int reset_units(size_t n) {
+    n_desc = std::max<size_t>(n, 1);
+    CUDA_TRY(units_dev.reserve_on(stream, n_desc * sizeof(UnitDesc)));
+    CUDA_TRY(h_units.reserve(n_desc * sizeof(UnitDesc)));
+    CUDA_TRY(unit_ctrs.reserve_on(stream, n_desc * 8));
+    CUDA_TRY(cudaMemsetAsync(unit_ctrs.p, 0, n_desc * 8, stream));
+    desc_block.assign(n_desc, 0);
+    return B2_OK;
+  }
+  UnitDesc& desc(size_t d) { return ((UnitDesc*)h_units.p)[d]; }
+  void set_desc(size_t d, const ScanArgs& a, uint32_t block_idx) {
+    UnitDesc& x = desc(d);
+    x.blk = a.blk; x.e_lo = a.e_lo; x.c_lo = a.c_lo; x.c_hi = a.c_hi; x.tile_lo = 0;
+    x.entry_base = a.entry_base; x.range_rows = a.range_rows; x.ck_key_state = a.ck_key_state; x.slow_off = 0;
+    desc_block[d] = block_idx;
+  }
+  int upload_units(size_t d_lo, size_t d_hi) {
+    CUDA_TRY(cudaMemcpyAsync((UnitDesc*)units_dev.p + d_lo, &desc(d_lo), (d_hi - d_lo) * sizeof(UnitDesc), cudaMemcpyHostToDevice, stream));
+    return B2_OK;
+  }
+  // tile_lo / slow_off of the descriptors [d_lo, d_hi) as one group: tiles and hand-over segments one after the other
+  void lay_out_group(size_t d_lo, size_t d_hi) {
+    uint32_t t = 0;
+    uint64_t s = 0;
+    for (size_t d = d_lo; d < d_hi; ++d) {
+      desc(d).tile_lo = t; desc(d).slow_off = s;
+      t += (desc(d).c_hi - desc(d).c_lo + TILE - 1) / TILE;
+      s += desc(d).c_hi - desc(d).c_lo;
     }
-    CUDA_TRY(slow_list.reserve_on(stream, (size_t)(u.e_hi - u.e_lo) * 4 + 16));
-    CUDA_TRY(slow_cnt.reserve_on(stream, 16));
-    CUDA_TRY(cudaMemsetAsync(slow_cnt.p, 0, 4, stream));
-    ScanArgs f = a0;
-    f.slow_list = (unsigned int*)slow_list.p; f.slow_count = (unsigned int*)slow_cnt.p;
+  }
+  // One lean launch over the uploaded descriptors [d_lo, d_hi), then scan_body in list mode over each one's hand-over
+  // segment.  args_of(d): the descriptor's unit arguments (mode pointers set).  fast_smem_mode: bytes of mode state in front
+  // of the stages; fast_slots: CTA table slots of the lean aggregation kernel.  TopN: topn_work is the lean kernel's
+  // candidate area, and the general kernel's too when general_smem_mode is 0 (the launches are stream-ordered).  *launched
+  // stays false when no stage can hold the group's tiles: the caller runs the general kernel over each unit instead.
+  template <class ArgsOf>
+  int launch_group(size_t d_lo, size_t d_hi, ArgsOf args_of, size_t general_smem_mode, size_t fast_smem_mode, uint32_t fast_slots, int* general_grid_out,
+                   int* fast_grid_out, bool* launched) {
+    *launched = false;
+    uint32_t n_tiles = 0;
+    uint64_t n_ent = 0;
+    for (size_t d = d_lo; d < d_hi; ++d) {
+      n_tiles += (desc(d).c_hi - desc(d).c_lo + TILE - 1) / TILE;
+      n_ent = std::max<uint64_t>(n_ent, desc(d).slow_off + desc(d).c_hi - desc(d).c_lo);
+    }
+    // stage capacities of the block with the largest entries (the capacity grows with the average entry size)
+    uint32_t big = desc_block[d_lo];
+    for (size_t d = d_lo; d < d_hi; ++d) {
+      const SrcBlock &x = wblocks[desc_block[d]], &y = wblocks[big];
+      if ((x.key_bytes + x.val_bytes) * std::max<uint64_t>(1, y.c.n) > (y.key_bytes + y.val_bytes) * std::max<uint64_t>(1, x.c.n)) big = desc_block[d];
+    }
+    ScanArgs f = args_of(d_lo);
     f.smem_slots = fast_slots;
-    size_t ftot = setup_staging(&f, wblocks[u.block_idx], fast_smem_mode);
+    size_t ftot = setup_staging(&f, wblocks[big], fast_smem_mode);
+    if (!f.staging) return B2_OK;  // no staging possible (huge entries): everything goes through the general kernel
+    CUDA_TRY(slow_list.reserve_on(stream, n_ent * 4 + 16));
+    f.slow_list = (unsigned int*)slow_list.p;
+    f.units = (const UnitDesc*)units_dev.p + d_lo; f.n_units = (uint32_t)(d_hi - d_lo); f.n_unit_tiles = n_tiles;
+    f.tile_ctr = (unsigned int*)unit_ctrs.p + d_lo; f.slow_count = (unsigned int*)unit_ctrs.p + n_desc + d_lo;
     const JitKernel* jk = jit_ready();
     if (jk && !jk->fn_fast) jk = nullptr;
     int fgrid = jk ? jit_max_blocks_per_sm(jk, ftot, JIT_FAST) * scan_num_sms() : fast_max_grid(cp.dev.mode, ftot);
     if (fast_grid_out && *fast_grid_out > 0) fgrid = std::min(fgrid, *fast_grid_out);
-    kernel_begin();
-    if (f.staging) {
-      if (jk) { stats.jit_launches++; CUDA_TRY(jit_launch(jk, f, fgrid, ftot, stream, JIT_FAST)); }
-      else CUDA_TRY(launch_fast(cp.dev, f, fgrid, ftot, stream));
-    } else {  // no staging possible (huge entries): everything goes through the general kernel
-      fast = false;
-    }
-    ScanArgs g = a0;
-    if (general_smem_mode) g.topn_work = nullptr;
-    size_t gtot = general_smem_mode;
-    if (fast) {
-      g.slow_list = f.slow_list; g.slow_count = f.slow_count; g.list_mode = 1;
+    const int mode = scan_kernel_mode(cp.dev);
+    kernel_begin();  // (the bracket covers the lean launch and every list-mode launch behind it)
+    if (jk) { stats.jit_launches++; CUDA_TRY(jit_launch(jk, f, fgrid, ftot, stream, JIT_FAST)); }
+    else CUDA_TRY(launch_fast(cp.dev, f, fgrid, ftot, stream));
+    int ggrid = 0;
+    for (size_t d = d_lo; d < d_hi; ++d) {
+      ScanArgs g = args_of(d);
+      if (general_smem_mode) g.topn_work = nullptr;
+      g.slow_list = f.slow_list + desc(d).slow_off; g.slow_count = f.slow_count + (d - d_lo); g.list_mode = 1;
       g.staging = 0; g.stage_off = 0; g.stage_key_cap = g.stage_val_cap = 0;
-    } else {
-      gtot = setup_staging(&g, wblocks[u.block_idx], general_smem_mode);
+      ggrid = general_grid_for(g, mode, general_smem_mode);
+      if (general_grid_out && *general_grid_out > 0) ggrid = std::min(ggrid, *general_grid_out);
+      if (cp.dev.mode == PM_TOPN) {  // the two kernels leave their per-CTA lists side by side
+        g.topn.items += (size_t)fgrid * g.topn.stride; g.topn.counts += fgrid;
+      }
+      CUDA_TRY(general_launch(g, mode, ggrid, general_smem_mode));
     }
-    int ggrid = general_grid_for(g, mode, gtot);
-    if (general_grid_out && *general_grid_out > 0) ggrid = std::min(ggrid, *general_grid_out);
-    if (cp.dev.mode == PM_TOPN && fast) {  // the two kernels leave their per-CTA lists side by side
-      g.topn.items = a0.topn.items + (size_t)fgrid * a0.topn.stride; g.topn.counts = a0.topn.counts + fgrid;
-    }
-    CUDA_TRY(general_launch(g, mode, ggrid, gtot));
     kernel_end();
-    stats.kernel_launches += fast ? 1 : 0;
+    stats.kernel_launches += d_hi - d_lo;  // (kernel_end counted one)
     if (general_grid_out) *general_grid_out = ggrid;
-    if (fast_grid_out) *fast_grid_out = fast ? fgrid : 0;
+    if (fast_grid_out) *fast_grid_out = fgrid;
+    *launched = true;
+    return B2_OK;
+  }
+  // Aggregation and checksum: every unit, in groups of one lean launch: over device-resident blocks one group, else the
+  // units of one staged block (two staging slots).  args_of(u, view): the unit's arguments; fast_of(u, &args): whether the
+  // unit takes the lean kernel (it may set the unit's ck_key_state); the other units run the general kernel.  Returns with
+  // `failed` set when the deadline passed before a launch.
+  template <class ArgsOf, class FastOf>
+  int run_units(ArgsOf args_of, FastOf fast_of, size_t general_smem, size_t fast_smem, uint32_t fast_slots, bool count_iterations) {
+    int rc = reset_units(units.size());
+    if (rc) return rc;
+    size_t nd = 0;
+    std::vector<ScanArgs> lean_args;
+    std::vector<std::pair<size_t, ScanArgs>> general;
+    for (size_t lo = 0; lo < units.size();) {
+      size_t hi = lo + 1;
+      if (src_loc == B2_LOC_DEVICE) hi = units.size();
+      else while (hi < units.size() && units[hi].block_idx == units[lo].block_idx) ++hi;
+      const size_t d_lo = nd;
+      lean_args.clear(); general.clear();
+      for (size_t ui = lo; ui < hi; ++ui) {
+        BlockView v;
+        rc = acquire_block(units[ui].block_idx, &v);
+        if (rc) return rc;
+        ScanArgs a = args_of(units[ui], v);
+        if (fast_of(units[ui], &a)) { set_desc(nd++, a, units[ui].block_idx); lean_args.push_back(a); }
+        else general.push_back({ui, a});
+      }
+      if (nd > d_lo) {
+        if (deadline_exceeded()) return B2_OK;
+        lay_out_group(d_lo, nd);
+        rc = upload_units(d_lo, nd);
+        if (rc) return rc;
+        bool launched = false;
+        rc = launch_group(d_lo, nd, [&](size_t d) { return lean_args[d - d_lo]; }, general_smem, fast_smem, fast_slots, nullptr, nullptr, &launched);
+        if (rc) return rc;
+        for (size_t d = d_lo; d < nd && !launched; ++d) {
+          rc = launch_general(lean_args[d - d_lo], desc_block[d], general_smem, nullptr);
+          if (rc) return rc;
+        }
+      }
+      for (auto& g : general) {
+        if (deadline_exceeded()) return B2_OK;
+        rc = launch_general(g.second, units[g.first].block_idx, general_smem, nullptr);
+        if (rc) return rc;
+      }
+      for (size_t ui = lo; ui < hi; ++ui) {
+        entries_scanned += units[ui].e_hi - units[ui].e_lo;
+        if (count_iterations) stats.num_iterations++;
+      }
+      release_block(units[lo].block_idx);
+      prefetch_after(hi - 1);
+      lo = hi;
+    }
     return B2_OK;
   }
 
@@ -1475,30 +1582,19 @@ struct b2_exec {
       if (rc) return rc;
       rc = init_device_state();
       if (rc) return rc;
-      int grid = 0;
-      size_t grid_smem = ~(size_t)0;
       entries_scanned = 0;
-      for (size_t ui = 0; ui < units.size(); ++ui) {
-        const Unit& u = units[ui];
-        if (deadline_exceeded()) { cudaStreamSynchronize(stream); return publish_agg(0, nullptr, nullptr, nullptr, out); }
-        BlockView v;
-        rc = acquire_block(u.block_idx, &v);
-        if (rc) return rc;
+      auto args_of = [&](const Unit& u, const BlockView& v) {
         ScanArgs a = base_args(u, v);
         a.c_lo = u.e_lo; a.c_hi = u.e_hi;
         a.tbl.keys = (unsigned long long*)tbl_keys.p; a.tbl.special = (unsigned int*)tbl_occ.p; a.tbl.acc = (unsigned long long*)tbl_acc.p; a.tbl.cap = tbl_cap;
         a.tbl.gkeys = (unsigned long long*)tbl_gkeys.p; a.tbl.ready = (unsigned int*)tbl_ready.p; a.tbl.hash_mask_bits = debug_hash_bits;
         a.smem_slots = smem_slots;
-        const bool fast = u.fast_ok && fast_kernel_covers();
-        int gg = 0, fg = 0;
-        rc = launch_unit(a, u, fast, smem, fast_smem, fast_slots, &gg, &fg);
-        if (rc) return rc;
-        grid = gg;
-        release_block(u.block_idx);
-        prefetch_after(ui);
-        entries_scanned += u.e_hi - u.e_lo;
-        stats.num_iterations++;
-      }
+        return a;
+      };
+      auto fast_of = [&](const Unit& u, ScanArgs*) { return u.fast_ok && fast_kernel_covers(); };
+      rc = run_units(args_of, fast_of, smem, fast_smem, fast_slots, true);
+      if (rc) return rc;
+      if (failed) { cudaStreamSynchronize(stream); return publish_agg(0, nullptr, nullptr, nullptr, out); }
       // the group table -> compact group list right behind the last unit, so that one read of the counters serves both;
       // the list of a table that overflowed is discarded with it
       if (P.has_group) {
@@ -1637,28 +1733,70 @@ struct b2_exec {
       // comparison.  The very first rows have no such bound, so the request starts with short chunks that grow 8x each:
       // after c rows the bound passes about limit / c of what follows, i.e. every chunk hands ~8 x limit candidates to
       // the merge below instead of one full list per CTA.
-      uint64_t seeded_rows = 0;
+      // The chunks are known in advance: each is a lean launch group of one descriptor.  The descriptors of all chunks are
+      // uploaded once (device-resident blocks) or once per unit, when its block has been staged.
+      std::vector<std::pair<uint32_t, uint32_t>> chunks;  // c_lo, c_hi
+      std::vector<size_t> unit_first_chunk(units.size() + 1, 0);
+      {
+        uint64_t seeded = 0;
+        for (size_t ui = 0; ui < units.size(); ++ui) {
+          unit_first_chunk[ui] = chunks.size();
+          for (uint32_t c_lo = units[ui].e_lo; c_lo < units[ui].e_hi;) {
+            const uint64_t want = std::max<uint64_t>(16 * TILE, 7 * seeded);
+            const uint32_t c_hi = (uint64_t)(units[ui].e_hi - c_lo) <= want + want / 2 ? units[ui].e_hi : c_lo + (uint32_t)want;
+            chunks.push_back({c_lo, c_hi});
+            seeded += c_hi - c_lo;
+            c_lo = c_hi;
+          }
+        }
+        unit_first_chunk[units.size()] = chunks.size();
+      }
+      rc = reset_units(chunks.size());
+      if (rc) return rc;
+      auto chunk_args = [&](size_t ui, const BlockView& v, size_t d) {
+        ScanArgs a = base_args(units[ui], v);
+        a.c_lo = chunks[d].first; a.c_hi = chunks[d].second;
+        return a;
+      };
       for (size_t ui = 0; ui < units.size(); ++ui) {
+        if (src_loc != B2_LOC_DEVICE || ui == 0) {
+          const size_t ui_hi = src_loc == B2_LOC_DEVICE ? units.size() : ui + 1;
+          for (size_t uj = ui; uj < ui_hi; ++uj) {
+            BlockView v;
+            rc = acquire_block(units[uj].block_idx, &v);
+            if (rc) return rc;
+            for (size_t d = unit_first_chunk[uj]; d < unit_first_chunk[uj + 1]; ++d) set_desc(d, chunk_args(uj, v, d), units[uj].block_idx);
+          }
+          if (unit_first_chunk[ui_hi] > unit_first_chunk[ui]) {
+            rc = upload_units(unit_first_chunk[ui], unit_first_chunk[ui_hi]);
+            if (rc) return rc;
+          }
+        }
        const Unit& u = units[ui];
        BlockView v;
        rc = acquire_block(u.block_idx, &v);
        if (rc) return rc;
-       for (uint32_t c_lo = u.e_lo; c_lo < u.e_hi;) {
+       for (size_t d = unit_first_chunk[ui]; d < unit_first_chunk[ui + 1]; ++d) {
         if (deadline_exceeded()) break;
-        const uint64_t want = std::max<uint64_t>(16 * TILE, 7 * seeded_rows);
-        const uint32_t c_hi = (uint64_t)(u.e_hi - c_lo) <= want + want / 2 ? u.e_hi : c_lo + (uint32_t)want;
-        ScanArgs a = base_args(u, v);
-        a.c_lo = c_lo; a.c_hi = c_hi;
+        const uint32_t c_lo = chunks[d].first, c_hi = chunks[d].second;
+        ScanArgs a = chunk_args(ui, v, d);
         uint32_t n_tiles = (c_hi - c_lo + TILE - 1) / TILE;
         a.topn.items = (TopItem*)tn_lists.p; a.topn.counts = (unsigned int*)tn_counts.p; a.topn.stride = limit;
         a.topn_cap = cap;
         a.topn_seed = run_items; a.topn_seed_cnt = run_cnt;
         a.topn_work = (unsigned char*)tn_work.p; a.topn_work_stride = buf_bytes;
         CUDA_TRY(cudaMemsetAsync(tn_counts.p, 0, (size_t)lists_cap * 4, stream));
-        const bool fast = any_fast && u.fast_ok;
         int gg = (int)std::min<uint32_t>((uint32_t)grid, n_tiles), fg = (int)std::min<uint32_t>((uint32_t)std::max(fast_grid, 1), n_tiles);
-        rc = launch_unit(a, u, fast, smem, 0, 0, &gg, &fg);
-        if (rc) return rc;
+        bool launched = false;
+        if (any_fast && u.fast_ok) {
+          rc = launch_group(d, d + 1, [&](size_t) { return a; }, smem, 0, 0, &gg, &fg, &launched);
+          if (rc) return rc;
+        }
+        if (!launched) {
+          fg = 0;
+          rc = launch_general(a, u.block_idx, smem, &gg);
+          if (rc) return rc;
+        }
         a.topn.n_lists = (uint32_t)(gg + fg);
         // unit top-N (sorted) lands in the second half of `pair`
         TopNLists unit_out; unit_out.items = unit_items; unit_out.counts = unit_cnt; unit_out.n_lists = 1; unit_out.stride = limit;
@@ -1682,10 +1820,8 @@ struct b2_exec {
                                   (const unsigned long long*)tn_blk_pay.p, (const unsigned char*)tn_blk_null.p, (unsigned long long*)nxt_pay->p, (unsigned char*)nxt_null->p, stream));
         std::swap(run_items, nxt_items); std::swap(run_cnt, nxt_cnt); std::swap(run_pay, nxt_pay); std::swap(run_null, nxt_null);
         entries_scanned += c_hi - c_lo;
-        seeded_rows += c_hi - c_lo;
         stats.num_iterations++;
         stats.kernel_launches += 4;
-        c_lo = c_hi;
        }
        release_block(u.block_idx);
        prefetch_after(ui);
@@ -2105,18 +2241,17 @@ int32_t b2_checksum_handle(const b2_key_range* ranges, uint32_t n_ranges, const 
   for (uint32_t i = 0; i < old_prefix_len; ++i) st = crc64_table_entry((uint8_t)(st ^ old_prefix[i])) ^ (st >> 8);
   if (new_prefix_len > 32) { g_last_error = "new_prefix longer than 32 bytes"; return B2_ERR_UNSUPPORTED; }
   h->cp.dev.read_ts = h->read_ts; h->cp.dev.isolation = h->isolation;
-  for (size_t ui = 0; ui < h->units.size(); ++ui) {
-    const Unit& u = h->units[ui];
-    BlockView v;
-    rc = h->acquire_block(u.block_idx, &v);
-    if (rc) return rc;
+  auto args_of = [&](const Unit& u, const BlockView& v) {
     ScanArgs a = h->base_args(u, v);
     a.c_lo = u.e_lo; a.c_hi = u.e_hi;
     a.ck_init_state = st; a.ck_new_prefix_len = new_prefix_len; a.ck_old_prefix_len = old_prefix_len;
     memcpy(a.ck_new_prefix, new_prefix, new_prefix_len);
-    // lean kernel: the unit's keys share their first 11 raw bytes ('t' table-id "_r"); the crc register after old_prefix and
-    // raw[new_prefix_len .. 11) is the same for all of them.  (A new_prefix that reaches into the handle, or that the
-    // unit's keys do not start with, is left to the general kernel, which also raises "Wrong prefix".)
+    return a;
+  };
+  // lean kernel: the unit's keys share their first 11 raw bytes ('t' table-id "_r"); the crc register after old_prefix and
+  // raw[new_prefix_len .. 11) is the same for all of them.  (A new_prefix that reaches into the handle, or that the
+  // unit's keys do not start with, is left to the general kernel, which also raises "Wrong prefix".)
+  auto fast_of = [&](const Unit& u, ScanArgs* a) {
     bool fast = u.fast_ok && h->fast_kernel_covers() && new_prefix_len <= 11;
     if (fast) {
       uint8_t raw[11];
@@ -2126,14 +2261,13 @@ int32_t b2_checksum_handle(const b2_key_range* ranges, uint32_t n_ranges, const 
       uint64_t ks = st;
       for (uint32_t j = 0; j < new_prefix_len && fast; ++j) fast = raw[j] == new_prefix[j];
       for (uint32_t j = new_prefix_len; j < 11; ++j) ks = crc64_table_entry((uint8_t)(ks ^ raw[j])) ^ (ks >> 8);
-      a.ck_key_state = ks;
+      a->ck_key_state = ks;
     }
-    rc = h->launch_unit(a, u, fast, scan_crc_table_bytes(), fast_checksum_bytes(), 0, nullptr, nullptr);
-    if (rc) return rc;
-    h->release_block(u.block_idx);
-    h->prefetch_after(ui);
-    h->entries_scanned += u.e_hi - u.e_lo;
-  }
+    return fast;
+  };
+  rc = h->run_units(args_of, fast_of, scan_crc_table_bytes(), fast_checksum_bytes(), 0, false);
+  if (rc) return rc;
+  if (h->failed) { cudaStreamSynchronize(h->stream); g_last_error = h->last_err.message; return h->last_err.status; }
   Counters c;
   rc = h->read_counters(&c);
   if (rc) return rc;

@@ -26,15 +26,22 @@ enum { FK_STAGES = 2, FK_THREADS = TILE + 32, CK_WORDS = 16 /* value bytes / 8 t
 
 __device__ __forceinline__ unsigned int hash32(unsigned long long k) { return ((unsigned int)k ^ (unsigned int)(k >> 32)) * 0x9E3779B1u; }
 
+// a stage's tile and what the decoding warps need of its unit (read from shared memory per tile, not held in registers)
+struct FastTileMeta : TileMeta {
+  uint32_t unit, e0, e_lo, c_hi;  // the unit's index, the tile's first entry, the unit's first entry and end
+  unsigned long long entry_base;
+  const uint8_t* gvals;
+};
+
 template <int MODE>
 __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
   static_assert(MODE == PM_AGG || MODE == PM_TOPN || MODE == PM_CHECKSUM, "order-free pipelines only");
   extern __shared__ __align__(16) unsigned char dyn_smem[];
   const unsigned int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const uint32_t n_tiles = (A.c_hi - A.c_lo + TILE - 1) / TILE;
+  const uint32_t n_tiles = A.n_unit_tiles;
 
   __shared__ __align__(8) unsigned long long s_full[FK_STAGES], s_empty[FK_STAGES];
-  __shared__ TileMeta s_meta[FK_STAGES];
+  __shared__ FastTileMeta s_meta[FK_STAGES];
   __shared__ unsigned int s_tbl_used, s_tbl_miss, s_tbl_off;
   __shared__ unsigned int s_top_cnt, s_top_have_thr, s_top_next_sync;
   __shared__ TopItem s_top_thr;
@@ -79,25 +86,42 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
   const uint32_t STAGE_KEY_CAP = A.stage_key_cap, STAGE_VAL_CAP = A.stage_val_cap;
   const uint32_t STAGE_BYTES = STAGE_KEY_CAP + STAGE_VAL_CAP + 2 * STAGE_OFF_CAP;
 
-  // ---- producer warp: bulk copies of each tile's key / value bytes and offset slices, FK_STAGES tiles ahead ----
+  // ---- producer warp: claims tiles of the unit table from one counter (so no CTA is left with a tail of its own), and
+  // issues bulk copies of each tile's key / value bytes and offset slices, FK_STAGES tiles ahead.  Software-pipelined by
+  // one tile: the claim and the four bounding offsets of tile k+1 are fetched while the producer waits for a free stage ----
   if (wid == TILE / 32) {
     if (lane == 0) {
+      uint32_t u = 0;  // cursor into the unit table: claims only increase
+      uint32_t nx_tile, nx_e0 = 0, nx_wlo = 0, nx_whi = 0, nx_k0 = 0, nx_k1 = 0, nx_v0 = 0, nx_v1 = 0;
+      auto claim = [&]() {
+        nx_tile = atomicAdd(A.tile_ctr, 1u);
+        if (nx_tile < n_tiles) {
+          while (u + 1 < A.n_units && A.units[u + 1].tile_lo <= nx_tile) ++u;
+          const UnitDesc& d = A.units[u];
+          nx_e0 = d.c_lo + (nx_tile - d.tile_lo) * TILE;
+          nx_whi = nx_e0 + TILE < d.c_hi ? nx_e0 + TILE : d.c_hi;
+          nx_wlo = nx_e0 > d.e_lo ? nx_e0 - 1 : nx_e0;
+          nx_k0 = d.blk.koff[nx_wlo]; nx_k1 = d.blk.koff[nx_whi]; nx_v0 = d.blk.voff[nx_wlo]; nx_v1 = d.blk.voff[nx_whi];
+        }
+      };
+      claim();
       for (uint32_t k = 0;; ++k) {
         const int slot = (int)(k % FK_STAGES);
-        TileMeta m;
-        m.tile = blockIdx.x + k * gridDim.x;
+        FastTileMeta m;
+        m.tile = nx_tile;
         m.staged = 0; m.w_lo = 0; m.w_hi = 0; m.keys_adj = 0; m.vals_adj = 0; m.koff_adj = 0; m.voff_adj = 0;
-        uint32_t tx = 0, w_lo = 0, w_hi = 0, k0 = 0, k1 = 0, v0 = 0, v1 = 0;
-        if (m.tile < n_tiles) {  // (the four bounding offsets are fetched before waiting for the stage)
-          const uint32_t e0 = A.c_lo + m.tile * TILE, e1 = e0 + TILE < A.c_hi ? e0 + TILE : A.c_hi;
-          w_lo = e0 > A.e_lo ? e0 - 1 : e0;
-          w_hi = e1;
-          k0 = A.blk.koff[w_lo]; k1 = A.blk.koff[w_hi]; v0 = A.blk.voff[w_lo]; v1 = A.blk.voff[w_hi];
+        m.unit = 0; m.e0 = 0; m.e_lo = 0; m.c_hi = 0; m.entry_base = 0; m.gvals = nullptr;
+        uint32_t tx = 0;
+        const uint32_t w_lo = nx_wlo, w_hi = nx_whi, k0 = nx_k0, k1 = nx_k1, v0 = nx_v0, v1 = nx_v1;
+        const BlockView blk = A.units[u].blk;
+        if (m.tile < n_tiles) {
+          const UnitDesc& d = A.units[u];
+          m.unit = u; m.e0 = nx_e0; m.e_lo = d.e_lo; m.c_hi = d.c_hi; m.entry_base = d.entry_base; m.gvals = d.blk.vals;
         }
         mbar_wait_sleep(&s_empty[slot], ((k / FK_STAGES) & 1) ^ 1);
         if (m.tile < n_tiles) {
-          unsigned long long ka = (unsigned long long)(A.blk.keys + k0), va = (unsigned long long)(A.blk.vals + v0);
-          unsigned long long oa = (unsigned long long)(A.blk.koff + w_lo), ob = (unsigned long long)(A.blk.voff + w_lo);
+          unsigned long long ka = (unsigned long long)(blk.keys + k0), va = (unsigned long long)(blk.vals + v0);
+          unsigned long long oa = (unsigned long long)(blk.koff + w_lo), ob = (unsigned long long)(blk.voff + w_lo);
           uint32_t kpad = (uint32_t)(ka & 15), vpad = (uint32_t)(va & 15), opad = (uint32_t)(oa & 15), qpad = (uint32_t)(ob & 15);
           uint32_t kbytes = (kpad + (k1 - k0) + 15) & ~15u, vbytes = (vpad + (v1 - v0) + 15) & ~15u;
           uint32_t obytes = (opad + (w_hi - w_lo + 1) * 4 + 15) & ~15u, qbytes = (qpad + (w_hi - w_lo + 1) * 4 + 15) & ~15u;
@@ -121,6 +145,7 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
           asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&s_full[slot])) : "memory");
         }
         if (m.tile >= n_tiles) break;
+        claim();
       }
     }
     return;
@@ -139,15 +164,36 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
 #pragma unroll
   for (int j = 0; j < (MODE == PM_CHECKSUM ? CK_WORDS : 1); ++j) vacc[j] = 0;
   const bool rc_check = A.isolation == B2_ISO_RC_CHECK_TS;
+  // rows returned and the last of them are per unit (its range's row count, its block's entry_base): the warp hands them
+  // over whenever its tile's unit changes (warp-uniform) and at the end
+  uint32_t w_unit = ~0u;
+  auto flush_unit = [&]() {
+    n_keys += n_keys32; n_keys32 = 0;
+    for (int off = 16; off > 0; off >>= 1) {
+      n_keys += __shfl_xor_sync(0xffffffffu, n_keys, off);
+      n_last = max(n_last, __shfl_xor_sync(0xffffffffu, n_last, off));
+    }
+    if (lane == 0) {
+      const UnitDesc& d = A.units[w_unit];
+      if (n_keys) atomicAdd(&A.ctr->processed_keys, n_keys);
+      if (n_keys && d.range_rows) atomicAdd(d.range_rows, n_keys);
+      if (n_last) atomicMax(&A.ctr->last_row, d.entry_base + n_last);
+    }
+    n_keys = 0; n_last = 0;
+  };
 
   for (uint32_t k = 0;; ++k) {
     const int cur = (int)(k % FK_STAGES);
     mbar_wait_sleep(&s_full[cur], (k / FK_STAGES) & 1);  // suspended by the hardware until the stage lands: polling cost 6 % of the kernel's issue slots
     const uint32_t tile = s_meta[cur].tile;
     if (tile >= n_tiles) break;
-    const uint32_t e_raw = A.c_lo + tile * TILE + tid;
-    const bool valid = e_raw < A.c_hi;
-    const uint32_t e = valid ? e_raw : A.c_hi - 1;
+    if (s_meta[cur].unit != w_unit) {
+      if (w_unit != ~0u) flush_unit();
+      w_unit = s_meta[cur].unit;
+    }
+    const uint32_t e_raw = s_meta[cur].e0 + tid;
+    const bool valid = e_raw < s_meta[cur].c_hi;
+    const uint32_t e = valid ? e_raw : s_meta[cur].c_hi - 1;
     bool push = false, live = false, cand = false;
     uint32_t push_e = e_raw;
     // per-mode values computed before the hand-over decision (an evaluation error turns the commit into a push)
@@ -167,7 +213,7 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
       sv.svals = stg + STAGE_KEY_CAP + s_meta[cur].vals_adj;
       sv.skoff = reinterpret_cast<const uint32_t*>(stg + STAGE_KEY_CAP + STAGE_VAL_CAP) + s_meta[cur].koff_adj;
       sv.svoff = reinterpret_cast<const uint32_t*>(stg + STAGE_KEY_CAP + STAGE_VAL_CAP + STAGE_OFF_CAP) + s_meta[cur].voff_adj;
-      sv.gvals = A.blk.vals;
+      sv.gvals = s_meta[cur].gvals;
       const uint32_t ko = sv.skoff[e], kl = sv.skoff[e + 1] - ko, vo = sv.svoff[e], vl = sv.svoff[e + 1] - vo;
       const uint8_t* kp = sv.skeys + ko;
       const uint8_t* vp = sv.svals + vo;
@@ -182,7 +228,7 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
       unsigned int px = __shfl_up_sync(0xffffffffu, ((unsigned int)(t.b >> 32) & 0xffffffu) | (k35 ? 1u << 24 : 0u) | (vis ? 1u << 25 : 0u), 1);
       // (on the clamped index: in a unit of one entry the lanes past the end hold that entry too, and looking one entry back
       //  from it would index the offsets with -1)
-      const bool first = e == A.e_lo;
+      const bool first = e == s_meta[cur].e_lo;
       if (lane == 0 && !first) {
         KeyTail q;
         const bool q35 = sv.klen(e - 1) == 35;
@@ -241,7 +287,8 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
             Value v0;
             ok = eval_expr(P, P.order[0].e, row, cells, &v0, nullptr) == 0;
             cand = ok && (P.topn_all_keys || !s_top_have_thr || first_key_may_beat(P, v0, s_top_thr));
-            if (cand) ok = make_item(P, row, cells, A.desc ? ~(A.entry_base + e) : A.entry_base + e, &item, &v0) == 0;
+            const unsigned long long id = s_meta[cur].entry_base + e;
+            if (cand) ok = make_item(P, row, cells, A.desc ? ~id : id, &item, &v0) == 0;
           }
         }
         if (!ok) { push = true; commit = false; }  // the general decoder / evaluator owns this run (and raises its error)
@@ -255,9 +302,9 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
     const unsigned int pm = __ballot_sync(0xffffffffu, push);
     if (pm) {
       unsigned int base = 0;
-      if (lane == 0) base = atomicAdd(A.slow_count, (unsigned int)__popc(pm));
+      if (lane == 0) base = atomicAdd(A.slow_count + w_unit, (unsigned int)__popc(pm));
       base = __shfl_sync(0xffffffffu, base, 0);
-      if (push) A.slow_list[base + __popc(pm & ((1u << lane) - 1u))] = push_e;
+      if (push) A.slow_list[A.units[w_unit].slow_off + base + __popc(pm & ((1u << lane) - 1u))] = push_e;
     }
     n_live += live ? 1u : 0u;
     if ((k & 0xfffu) == 0xfffu) { n_keys += n_keys32; n_size += n_size32; n_keys32 = 0; n_size32 = 0; }  // (a lane adds < 2^20 per 4096 tiles)
@@ -276,7 +323,7 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
                 const unsigned long long key = has ? extremum_key(av[a].bits, g.arg_et, g.arg_unsigned, g.kind == AGG_MIN) : 0ull;
                 r_lo[a] = key > r_lo[a] ? key : r_lo[a];
               } else if (g.kind == AGG_FIRST) {  // r_lo / r_hi: the lane's (key, value) pair
-                const unsigned long long key = first_agg_key(A.entry_base + e, A.desc, !has);
+                const unsigned long long key = first_agg_key(s_meta[cur].entry_base + e, A.desc, !has);
                 if (key > r_lo[a]) { r_lo[a] = key; r_hi[a] = has ? av[a].bits : 0ull; }
               } else if (agg_is_bit(g.kind)) {
                 const unsigned long long x = bit_agg_word(g.kind, has, av[a].bits);
@@ -332,7 +379,7 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
                   }
                 if (commit_w) { atomicAdd(&w[0], (unsigned long long)cnt); atomicMax(&w[1], key); }
               } else if (g.kind == AGG_FIRST) {
-                unsigned long long key = first_agg_key(A.entry_base + e, A.desc, !has), val = has ? av[a].bits : 0ull;
+                unsigned long long key = first_agg_key(s_meta[cur].entry_base + e, A.desc, !has), val = has ? av[a].bits : 0ull;
                 if (!solo)
                   for (unsigned int mm = peers & (peers - 1); mm; mm &= mm - 1) {
                     const unsigned long long ok2 = __shfl_sync(peers, key, __ffs(mm) - 1), ov = __shfl_sync(peers, val, __ffs(mm) - 1);
@@ -382,7 +429,7 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
     } else {  // PM_CHECKSUM
       const unsigned int cm = __ballot_sync(0xffffffffu, live);
       if (cm) {
-        const unsigned long long ck = live ? crc_step8(crc_tab, A.ck_key_state, key_tail_handle_le(kw_a, kw_b)) : 0ull;
+        const unsigned long long ck = live ? crc_step8(crc_tab, A.units[w_unit].ck_key_state, key_tail_handle_le(kw_a, kw_b)) : 0ull;
         // the key states are folded per value length (the zero-byte advance by that length happens once, at the end)
         const uint32_t lead_len = __shfl_sync(0xffffffffu, rlen, __ffs(cm) - 1);
         if (__all_sync(0xffffffffu, !live || rlen == lead_len)) {
@@ -491,19 +538,15 @@ __device__ __forceinline__ void fast_body(const DevPlan& P, const ScanArgs& A) {
     }
   }
   // statistics
-  n_keys += n_keys32; n_size += n_size32;
+  if (w_unit != ~0u) flush_unit();
+  n_size += n_size32;
   for (int off = 16; off > 0; off >>= 1) {
-    n_keys += __shfl_xor_sync(0xffffffffu, n_keys, off);
     n_size += __shfl_xor_sync(0xffffffffu, n_size, off);
     n_live += __shfl_xor_sync(0xffffffffu, n_live, off);
     n_newer |= __shfl_xor_sync(0xffffffffu, n_newer, off);
-    n_last = max(n_last, __shfl_xor_sync(0xffffffffu, n_last, off));
     n_warn += __shfl_xor_sync(0xffffffffu, n_warn, off);
   }
   if (lane == 0) {
-    if (n_keys) atomicAdd(&A.ctr->processed_keys, n_keys);
-    if (n_keys && A.range_rows) atomicAdd(A.range_rows, n_keys);
-    if (n_last) atomicMax(&A.ctr->last_row, A.entry_base + n_last);
     if (n_size) atomicAdd(&A.ctr->processed_size, n_size);
     if (n_live) atomicAdd(&A.ctr->live_rows, n_live);
     if (n_newer) atomicOr(&A.ctr->met_newer, 1u);

@@ -57,6 +57,19 @@ struct TopNLists {
   unsigned int n_lists, stride;
 };
 
+// One unit of a lean launch (fast_kernel.cuh): the launch walks the tiles of a table of these, claimed from one counter.
+// Tiles never straddle units.
+struct UnitDesc {
+  BlockView blk;
+  uint32_t e_lo;                    // first entry of the unit (the look-back of its first tile stops there)
+  uint32_t c_lo, c_hi;              // the entries this launch covers (runs *starting* in [c_lo, c_hi))
+  uint32_t tile_lo;                 // tiles of the units before this one in the table
+  uint64_t entry_base;              // global index of blk entry 0
+  unsigned long long* range_rows;   // the unit's scanned_rows_per_range slot, or nullptr
+  uint64_t ck_key_state;            // checksum: see ScanArgs::ck_key_state
+  uint64_t slow_off;                // the unit's segment of ScanArgs::slow_list
+};
+
 struct ScanArgs {
   BlockView blk;
   DefaultCf dflt;
@@ -105,6 +118,12 @@ struct ScanArgs {
   unsigned char* topn_work;           // lean TopN kernel: the CTAs' candidate buffers live in HBM / L2 (topn_work + blockIdx.x * stride): a
   unsigned long long topn_work_stride;//   seeded CTA touches its buffer for a handful of rows per launch, and shared memory buys a third CTA per SM.
                                       //   Above LIMIT 2048 the general kernel's buffers live there too (scan_topn_hbm_kernel)
+  // the lean kernel: its units (it reads none of blk, e_lo, c_lo, c_hi, entry_base, range_rows, ck_key_state above), the
+  // counter its CTAs claim tiles from (zeroed before the launch), and per unit a hand-over count (slow_count[u]) and segment
+  // (slow_list + units[u].slow_off)
+  const UnitDesc* units;
+  unsigned int* tile_ctr;
+  uint32_t n_units, n_unit_tiles;
 };
 
 struct GenArgs {
