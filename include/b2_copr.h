@@ -494,10 +494,12 @@ int32_t b2_region_unpin(int32_t device, uint64_t region_id, uint64_t data_versio
 void b2_region_cache_stats(int32_t device, uint64_t* bytes_cached, uint64_t* hits, uint64_t* misses);
 
 /* ---- RocksDB data blocks as the data source (SURVEY.md §8(f)4: the on-disk block reader) -----------------------------
- * TiKV's block cache holds *uncompressed* BlockBasedTable data blocks whose keys are prefix-compressed between restart
- * points (RocksDB is an external dependency of the reference; block size and format version come from
- * src/config/mod.rs:966 and :704).  b2_sst_decode takes a run of such blocks, in key order, and expands them on the
- * device into the flat b2_cf_block layout the scan kernels read: the bytes that cross PCIe are the compressed ones.
+ * BlockBasedTable data blocks keep their keys prefix-compressed between restart points (RocksDB is an external
+ * dependency of the reference; block size and format version come from src/config/mod.rs:966 and :704).  TiKV's block
+ * cache holds them uncompressed; in the file, levels 2-4 of the write and default CFs store them LZ4-compressed
+ * (src/config/mod.rs:981-988).  b2_sst_decode takes a run of such blocks, in key order, inflates the LZ4 ones and
+ * expands all of them on the device into the flat b2_cf_block layout the scan kernels read: the bytes that cross PCIe are
+ * the compressed ones.
  *
  *   data block  := entry* restart[u32 LE x num_restarts] num_restarts[u32 LE]   (+ 5-byte trailer: type, checksum)
  *   entry       := varint32 shared | varint32 non_shared | varint32 value_len | key[shared..] | value
@@ -506,8 +508,20 @@ void b2_region_cache_stats(int32_t device, uint64_t* bytes_cached, uint64_t* hit
  *
  * Supported: binary-search data blocks (no hash index: top bit of num_restarts clear), value type kTypeValue (1) in every
  * footer -- i.e. files that hold one RocksDB version of each key (bottommost level, ingested SSTs).  Anything else
- * answers B2_ERR_UNSUPPORTED and the host keeps its merging iterator.  Compressed blocks (LZ4 / ZSTD / Snappy) must be
- * uncompressed by the caller (the block cache already did).  Checksums of the trailer are not verified.              */
+ * answers B2_ERR_UNSUPPORTED and the host keeps its merging iterator.  Checksums of the trailer are not verified.
+ *
+ * Compression (trailer_len == 5 only: the trailer's first byte is RocksDB's compression type; with trailer_len == 0 the
+ * contents are plain):
+ *   0 kNoCompression        the contents are the data block
+ *   4 kLZ4Compression,      the contents are  varint32 uncompressed_size | LZ4 block  (format_version >= 2 framing; the
+ *   5 kLZ4HCCompression     raw LZ4 block format, no frame header): inflated on the device.  A declared size below 4,
+ *                           above 255 x the LZ4 bytes or above 1 GiB, or a stream that does not produce exactly that many
+ *                           bytes from exactly its bytes, is a corrupted block (B2_ERR_STORAGE)
+ *   1, 2, 3, 6, 7, 0x40,    Snappy, zlib, BZip2, Xpress, ZSTD and RocksDB's custom-compressor range: B2_ERR_UNSUPPORTED,
+ *   0x80 .. 0xfe            a valid block the host's reader may inflate
+ *   any other value         (8..0x3f, 0x41..0x7f, 0xff) no RocksDB writer stores it: a corrupted block (B2_ERR_STORAGE)
+ * Plain and LZ4 blocks may mix in one run.  Blocks compressed with a dictionary (CompressionOptions::max_dict_bytes > 0)
+ * carry no mark of it in the block: the caller must not pass them (TiKV's default sets no dictionary at the LZ4 levels). */
 typedef struct b2_sst_blocks {
   const uint8_t* data;        /* the blocks, back to back or with gaps; host or device memory (see `location`) */
   const uint64_t* block_offs; /* host memory, n_blocks + 1 ascending offsets into data: block b = [block_offs[b], block_offs[b+1])
@@ -521,9 +535,9 @@ typedef struct b2_sst_blocks {
 typedef struct b2_sst_stats {
   uint64_t n_entries, key_bytes, val_bytes; /* of the decoded block */
   uint64_t n_restart_intervals;
-  uint64_t h2d_bytes;                       /* compressed bytes + offsets copied host -> device by this call */
-  float decode_ms;                          /* device time of the expansion kernels (CUDA events) */
-  uint32_t _pad;
+  uint64_t h2d_bytes;                       /* block bytes as passed (LZ4 blocks compressed) + offsets copied host -> device */
+  float decode_ms;                          /* device time of the inflate and expansion kernels (CUDA events) */
+  uint32_t n_lz4_blocks;                    /* LZ4 / LZ4HC blocks inflated by this call */
 } b2_sst_stats;
 
 typedef struct b2_sst b2_sst; /* owner of the decoded device block */

@@ -6,16 +6,23 @@
 //   entry      := varint32 shared | varint32 non_shared | varint32 value_len | key bytes [shared, shared + non_shared) | value
 //   restart[j] := offset of an entry with shared == 0; one every block_restart_interval entries (16 by default)
 //
-// A restart interval is the unit of parallelism: one thread walks one interval (<= 16 entries in practice).  Three passes,
+// A restart interval is the unit of parallelism: one thread walks one interval (<= 16 entries in practice).  The passes,
 // each bounded by HBM traffic that is a small multiple of the block bytes:
-//   sst_restarts  one thread per data block: reads the footer, validates it           -> restart points per block
+//   sst_blocks    one thread per data block: the trailer's compression type, the slice; a plain block (type 0) gets its
+//                 contents view (the slice) and its footer read and validated   -> restart points per block; an LZ4 /
+//                 LZ4HC block (type 4 / 5) its framing checked                  -> inflated size per block
+//   sst_inflate   only when the run holds LZ4 blocks: one warp per LZ4 block (lz4_block.h) inflates it into the
+//                 handle's inflate buffer at the exclusive sum of the inflated sizes; that is its contents view.  sst_blocks
+//                 then reads the footers of the inflated blocks (the one extra host round trip, for compressed runs only)
 //   sst_count     one thread per restart interval: entries, key bytes, value bytes   -> prefix sums give every
 //                 interval its place in the flat block
 //   sst_expand    one warp per restart interval: the current key lives in the warp's registers (byte j in lane j % 32),
 //                 every entry overwrites the bytes past `shared` and streams the key, minus the data prefix and the
 //                 internal-key footer (whose value type must be kTypeValue), and the value out as consecutive bytes
-// The expansion runs an order of magnitude above the PCIe link the compressed bytes arrive over, which is the point:
-// fewer bytes cross the link (53 instead of 69 per C3 entry).
+// sst_count and sst_expand read each block through its contents view, so plain and LZ4 blocks mix in one run (RocksDB
+// stores a block plain when LZ4 saves less than 1/8 of it).  The expansion runs an order of magnitude above the PCIe
+// link the compressed bytes arrive over, which is the point: fewer bytes cross the link (53 instead of 69 per C3 entry
+// with prefix compression alone; LZ4 blocks of the same table hold about 0.31 of those bytes).
 #include <cub/cub.cuh>
 #include <cuda_runtime.h>
 
@@ -26,6 +33,7 @@
 #include <vector>
 
 #include "../../include/b2_copr.h"
+#include "lz4_block.h"
 
 namespace b2 {
 void set_last_error(const std::string& m);  // engine.cu (thread-local message behind b2_last_error_message)
@@ -38,8 +46,18 @@ enum { SST_OK = 0, SST_CORRUPT = 1, SST_UNSUPPORTED = 2 };
 struct SstView {
   const uint8_t* data;
   const unsigned long long* boffs;  // n_blocks + 1
+  const uint8_t* inflated;          // the inflated LZ4 blocks
+  const unsigned long long* voff;   // n_blocks: contents view of each block: offset into data, or into inflated | kInflated
+  const unsigned int* vlen;         // n_blocks: contents length (0: no view, the block failed its checks)
   unsigned int n_blocks, trailer, pl, sl;
 };
+constexpr unsigned long long kInflated = 1ull << 63;
+
+// (an offset, not a pointer, in the view array: with a pointer loaded from memory ptxas spills in sst_expand_kernel)
+__device__ __forceinline__ const uint8_t* view_of(const SstView& S, unsigned int b) {
+  const unsigned long long v = S.voff[b];
+  return (v & kInflated ? S.inflated : S.data) + (v & ~kInflated);
+}
 
 __device__ __forceinline__ unsigned int ld_le32(const uint8_t* p) { return (unsigned int)p[0] | ((unsigned int)p[1] << 8) | ((unsigned int)p[2] << 16) | ((unsigned int)p[3] << 24); }
 
@@ -57,21 +75,69 @@ __device__ __forceinline__ unsigned int get_var32(const uint8_t* p, const uint8_
 
 __device__ __forceinline__ void raise(unsigned int* err, unsigned int code) { atomicMax(err, code); }
 
-__global__ void sst_restarts_kernel(SstView S, unsigned int* nres /* n_blocks + 1, last = 0 */, unsigned int* err) {
+// restart count of a block from its contents view (0 and an error when the footer is invalid)
+__device__ __forceinline__ unsigned int block_restarts(const uint8_t* base, unsigned int len, unsigned int* err) {
+  if (len < 4) { raise(err, SST_CORRUPT); return 0; }
+  const unsigned int foot = ld_le32(base + len - 4);
+  if (foot >> 31) { raise(err, SST_UNSUPPORTED); return 0; }  // data block hash index packed into the footer
+  if (foot == 0 || (unsigned long long)foot * 4 + 4 > len) { raise(err, SST_CORRUPT); return 0; }
+  return foot;
+}
+
+struct ViewOut { unsigned long long* off; unsigned int* len; };  // the writable side of SstView::voff / vlen
+
+// RocksDB CompressionType values a valid block may carry that are not LZ4's stream format: the built-in Snappy 1, zlib 2,
+// BZip2 3, Xpress 6, ZSTD 7 and 0x40 (kZSTDNotFinalCompression, older files), and the custom-compressor range
+// 0x80..0xfe.  The host's block reader may inflate them: B2_ERR_UNSUPPORTED.  No RocksDB writer stores any other value
+// (8..0x3f, 0x41..0x7f, 0xff kDisableCompressionOption): a block carrying one is damaged.
+__device__ __forceinline__ bool host_compression(unsigned int t) { return (t >= 1 && t <= 7) || t == 0x40 || (t >= 0x80 && t <= 0xfe); }
+
+// Before inflation (inflated == 0): classify every block.  Plain blocks get their contents view and restart count, LZ4
+// blocks their declared size in isz (0 for every other block) and a restart count of 0; their number and the sum of
+// their sizes come back with the first round trip, so the inflate buffer is sized without another.  After inflation:
+// the restart count of every block from its view.
+__global__ void sst_blocks_kernel(SstView S, ViewOut V, unsigned int* nres /* n_blocks + 1, last = 0 */, unsigned long long* isz /* n_blocks + 1 */,
+                                  unsigned int* n_lz4, unsigned long long* lz4_bytes, unsigned int inflated, unsigned int* err) {
   const unsigned int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b > S.n_blocks) return;
-  if (b == S.n_blocks) { nres[b] = 0; return; }
+  if (b == S.n_blocks) { nres[b] = 0; if (!inflated) isz[b] = 0; return; }
+  if (inflated) { nres[b] = S.vlen[b] ? block_restarts(view_of(S, b), S.vlen[b], err) : 0; return; }
   const unsigned long long lo = S.boffs[b], hi = S.boffs[b + 1];
   unsigned int nr = 0;
+  unsigned long long sz = 0;
+  unsigned int len = 0, vlen = 0;
   if (hi < lo || hi - lo < (unsigned long long)S.trailer + 4 || hi - lo > 0xffffff00ull) raise(err, SST_CORRUPT);
   else {
-    const unsigned int len = (unsigned int)(hi - lo) - S.trailer;
-    const unsigned int foot = ld_le32(S.data + lo + len - 4);
-    if (foot >> 31) raise(err, SST_UNSUPPORTED);  // data block hash index packed into the footer
-    else if (foot == 0 || (unsigned long long)foot * 4 + 4 > len) raise(err, SST_CORRUPT);
-    else nr = foot;
+    const uint8_t* base = S.data + lo;
+    len = (unsigned int)(hi - lo) - S.trailer;
+    const unsigned int type = S.trailer ? base[len] : 0;  // the trailer's first byte: RocksDB's compression type
+    if (type == 0) { vlen = len; nr = block_restarts(base, len, err); }
+    else if (type == 4 || type == 5) {
+      unsigned int n, at;
+      if (b2lz4::frame(base, len, &n, &at)) { sz = n; atomicAdd(n_lz4, 1u); atomicAdd(lz4_bytes, sz); }
+      else raise(err, SST_CORRUPT);
+    } else raise(err, host_compression(type) ? SST_UNSUPPORTED : SST_CORRUPT);
   }
-  nres[b] = nr;
+  V.off[b] = lo; V.len[b] = vlen;
+  nres[b] = nr; isz[b] = sz;
+}
+
+// One warp per block: LZ4 blocks (isz[b + 1] > isz[b]) inflate into inflated + isz[b] and get that as their view.
+__global__ void __launch_bounds__(256) sst_inflate_kernel(SstView S, ViewOut V, const unsigned long long* isz /* exclusive sums */, unsigned int* err) {
+  const unsigned int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (b >= S.n_blocks) return;
+  const unsigned long long at = isz[b], size = isz[b + 1] - at;
+  if (size == 0) return;
+  const uint8_t* base = S.data + S.boffs[b];
+  const unsigned int len = (unsigned int)(S.boffs[b + 1] - S.boffs[b]) - S.trailer;
+  unsigned int n, p;
+  b2lz4::frame(base, len, &n, &p);  // (validated by sst_blocks_kernel: n == size)
+  uint8_t* out = (uint8_t*)S.inflated + at;
+  const bool ok = b2lz4::inflate(base + p, len - p, out, n, lane, 32);
+  if (lane == 0) {
+    if (ok) { V.off[b] = kInflated | at; V.len[b] = n; }
+    else raise(err, SST_CORRUPT);  // (no view: the footer pass must not read a half-written block and report its garbage)
+  }
 }
 
 struct Interval { const uint8_t *p, *end; };
@@ -81,8 +147,8 @@ __device__ __forceinline__ bool interval_of(const SstView& S, const unsigned int
   unsigned int lo = 0, hi = S.n_blocks;  // last block with ibase[b] <= t
   while (hi - lo > 1) { const unsigned int mid = (lo + hi) >> 1; if (ibase[mid] <= t) lo = mid; else hi = mid; }
   const unsigned int b = lo, j = t - ibase[b], nr = ibase[b + 1] - ibase[b];
-  const uint8_t* base = S.data + S.boffs[b];
-  const unsigned int len = (unsigned int)(S.boffs[b + 1] - S.boffs[b]) - S.trailer;
+  const uint8_t* base = view_of(S, b);
+  const unsigned int len = S.vlen[b];
   const unsigned int ents_end = len - 4 - 4 * nr;
   const uint8_t* rs = base + ents_end;
   const unsigned int s = ld_le32(rs + 4 * j), e = j + 1 < nr ? ld_le32(rs + 4 * (j + 1)) : ents_end;
@@ -317,6 +383,7 @@ struct b2_sst {
   RawBuf keys, koff, vals, voff;  // decoded block (b2_sst_decode)
   RawBuf enc, enc_offs;           // encoded blocks (b2_sst_encode)
   RawBuf boffs, nres, cnt_n, cnt_k, cnt_v, tmp, err;  // offsets, restart / entry counts and their prefix sums
+  RawBuf view_off, view_len, isz, inflated;           // contents views; inflated sizes and bytes of LZ4 blocks
   // (the buffers are freed after this, when the handle is deleted: the device is current and the stream drained by then)
   void destroy() {
     cudaSetDevice(device);
@@ -374,7 +441,9 @@ int check_err(b2_sst* s, b2_sst& w, const char* what) {
   unsigned int code = 0;
   SST_TRY(cudaMemcpyAsync(&code, w.err.p, 4, cudaMemcpyDeviceToHost, s->stream));
   SST_TRY(cudaStreamSynchronize(s->stream));
-  if (code == SST_UNSUPPORTED) return sst_fail(B2_ERR_UNSUPPORTED, std::string("b2_sst_decode: ") + what + ": data-block hash index or an entry whose value type is not kTypeValue");
+  if (code == SST_UNSUPPORTED)
+    return sst_fail(B2_ERR_UNSUPPORTED, std::string("b2_sst_decode: ") + what +
+                                            ": a block compressed other than LZ4 / LZ4HC, a data-block hash index or an entry whose value type is not kTypeValue");
   if (code) return sst_fail(B2_ERR_STORAGE, std::string("b2_sst_decode: ") + what + ": corrupted data block");
   return B2_OK;
 }
@@ -403,7 +472,10 @@ int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in,
   for (uint32_t b = 0; b <= nb && nb; ++b) rel[b] = in->block_offs[b] - lo;
   SST_TRY(cudaMemcpyAsync(w.boffs.p, rel.data(), rel.size() * 8, cudaMemcpyHostToDevice, s->stream));
   h2d += rel.size() * 8;
+  SST_TRY(w.view_off.reserve(((size_t)nb + 1) * 8)); SST_TRY(w.view_len.reserve(((size_t)nb + 1) * 4));
   SstView S;
+  const ViewOut V{(unsigned long long*)w.view_off.p, (unsigned int*)w.view_len.p};
+  S.inflated = nullptr; S.voff = V.off; S.vlen = V.len;
   S.boffs = (const unsigned long long*)w.boffs.p; S.n_blocks = nb; S.trailer = in->trailer_len; S.pl = in->key_prefix_len; S.sl = in->key_suffix_len;
   struct StagingHold {  // released on every return path
     Staging* st = nullptr;
@@ -417,14 +489,29 @@ int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in,
     S.data = (const uint8_t*)hold.st->buf.p;
   } else S.data = in->data + lo;
   SST_TRY(cudaEventRecord(s->ev0, s->stream));
-  uint32_t n_iv = 0, n_ent = 0;
+  uint32_t n_iv = 0, n_ent = 0, n_lz4 = 0;
   uint64_t kb = 0, vb = 0;
   if (nb) {
-    SST_TRY(w.nres.reserve(((size_t)nb + 1) * 4));
-    sst_restarts_kernel<<<(nb + 1 + 255) / 256, 256, 0, s->stream>>>(S, (unsigned int*)w.nres.p, (unsigned int*)w.err.p);
+    unsigned int* err = (unsigned int*)w.err.p;  // [0] error code, [1] LZ4 blocks, [2..3] their inflated bytes (u64)
+    unsigned long long* lz4_bytes = (unsigned long long*)(err + 2);
+    uint64_t total = 0;
+    SST_TRY(w.nres.reserve(((size_t)nb + 1) * 4)); SST_TRY(w.isz.reserve(((size_t)nb + 1) * 8));
+    sst_blocks_kernel<<<(nb + 1 + 255) / 256, 256, 0, s->stream>>>(S, V, (unsigned int*)w.nres.p, (unsigned long long*)w.isz.p, err + 1, lz4_bytes, 0, err);
     if ((rc = scan_inplace(s, w, (unsigned int*)w.nres.p, (size_t)nb + 1))) return rc;
     SST_TRY(cudaMemcpyAsync(&n_iv, (unsigned int*)w.nres.p + nb, 4, cudaMemcpyDeviceToHost, s->stream));
+    SST_TRY(cudaMemcpyAsync(&n_lz4, err + 1, 4, cudaMemcpyDeviceToHost, s->stream));
+    SST_TRY(cudaMemcpyAsync(&total, lz4_bytes, 8, cudaMemcpyDeviceToHost, s->stream));
     if ((rc = check_err(s, w, "block footers"))) return rc;
+    if (n_lz4) {  // inflate the LZ4 blocks, then count the restarts of every block again from the views: one more round trip
+      if ((rc = scan_inplace(s, w, (unsigned long long*)w.isz.p, (size_t)nb + 1))) return rc;
+      SST_TRY(w.inflated.reserve((size_t)total + 16));
+      S.inflated = (const uint8_t*)w.inflated.p;
+      sst_inflate_kernel<<<(unsigned int)(((size_t)nb + 7) / 8), 256, 0, s->stream>>>(S, V, (const unsigned long long*)w.isz.p, err);
+      sst_blocks_kernel<<<(nb + 1 + 255) / 256, 256, 0, s->stream>>>(S, V, (unsigned int*)w.nres.p, nullptr, nullptr, nullptr, 1, err);
+      if ((rc = scan_inplace(s, w, (unsigned int*)w.nres.p, (size_t)nb + 1))) return rc;
+      SST_TRY(cudaMemcpyAsync(&n_iv, (unsigned int*)w.nres.p + nb, 4, cudaMemcpyDeviceToHost, s->stream));
+      if ((rc = check_err(s, w, "LZ4 blocks"))) return rc;
+    }
     if (n_iv >= 0x7ffffff0u) return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_decode: too many restart intervals in one call: pass fewer data blocks");
     SST_TRY(w.cnt_n.reserve(((size_t)n_iv + 1) * 4)); SST_TRY(w.cnt_k.reserve(((size_t)n_iv + 1) * 8)); SST_TRY(w.cnt_v.reserve(((size_t)n_iv + 1) * 8));
     sst_count_kernel<<<(n_iv + 1 + 127) / 128, 128, 0, s->stream>>>(S, (const unsigned int*)w.nres.p, n_iv, (unsigned int*)w.cnt_n.p, (unsigned long long*)w.cnt_k.p,
@@ -459,6 +546,7 @@ int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in,
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_entries = n_ent; stats->key_bytes = kb; stats->val_bytes = vb; stats->n_restart_intervals = n_iv; stats->h2d_bytes = h2d;
+    stats->n_lz4_blocks = n_lz4;
     cudaEventElapsedTime(&stats->decode_ms, s->ev0, s->ev1);
   }
   return B2_OK;

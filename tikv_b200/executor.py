@@ -306,8 +306,9 @@ class DeviceRegion:
 
 
 class SstDecoder:
-    """b2_sst_decode: a run of RocksDB data blocks (uncompressed, prefix-compressed keys) -> a device-resident flat CF
-    block owned by this object.  `data` is a host buffer (bytes / numpy uint8 / address) or a device address."""
+    """b2_sst_decode: a run of RocksDB data blocks (prefix-compressed keys; stored plain or LZ4 / LZ4HC-compressed, the
+    type in each block's trailer) -> a device-resident flat CF block owned by this object.  `data` is a host buffer
+    (bytes / numpy uint8 / address) or a device address."""
 
     def __init__(self, device=0):
         self.device, self.h = device, C.c_void_p()
@@ -342,8 +343,9 @@ class SstDecoder:
 
 
 class SstRegion:
-    """A region source whose CF_WRITE blocks arrive as RocksDB data blocks: each (data, block_offs) run is expanded on
-    the device (b2_sst_decode) and the request reads the decoded blocks from HBM.  The other fields follow `like`."""
+    """A region source whose CF_WRITE blocks arrive as RocksDB data blocks: each (data, block_offs) run, plain or LZ4
+    blocks as stored, is inflated and expanded on the device (b2_sst_decode) and the request reads the decoded blocks
+    from HBM.  The other fields follow `like`."""
 
     def __init__(self, like, runs, device=0, **fmt):
         self._dec = [SstDecoder(device) for _ in runs]

@@ -160,7 +160,7 @@ class SstBlocks(C.Structure):
 
 class SstStats(C.Structure):
     _fields_ = [("n_entries", C.c_uint64), ("key_bytes", C.c_uint64), ("val_bytes", C.c_uint64), ("n_restart_intervals", C.c_uint64),
-                ("h2d_bytes", C.c_uint64), ("decode_ms", C.c_float), ("_pad", C.c_uint32)]
+                ("h2d_bytes", C.c_uint64), ("decode_ms", C.c_float), ("n_lz4_blocks", C.c_uint32)]
 
 
 class SstEncoded(C.Structure):
