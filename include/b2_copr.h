@@ -462,6 +462,21 @@ int32_t b2_exec_agg_partials(b2_exec* h, b2_agg_partials* out);
  * is.  *n_inout: capacity of `ops` in, acc_words out (B2_ERR_INVALID_ARG when the capacity is smaller). */
 enum { B2_MERGE_ADD = 0, B2_MERGE_MAX = 1, B2_MERGE_OR = 2, B2_MERGE_XOR = 3, B2_MERGE_FIRST_KEY = 4, B2_MERGE_FIRST_VALUE = 5 };
 int32_t b2_exec_agg_word_ops(b2_exec* h, uint8_t* ops, uint32_t* n_inout);
+/* Final merge of partial tables gathered from several requests / GPUs, on the device.  n_rows rows (< 2^31), on
+ * `device`: row r has key_words (1..4) key words keys[r * keys_stride + k], the NULL mask key_null[r] (bit q = q-th key
+ * is NULL, below 2^key_words) and acc_words state words acc[r * acc_stride + w] (strides in words).  The rows of part p
+ * are [part_offs[p], part_offs[p + 1]) (host array, n_parts + 1 offsets from 0 to n_rows).  A group is a distinct
+ * (NULL mask, key words); with one key word a NULL row's key bits do not count.  Groups come out sorted ascending by the
+ * NULL mask, then by the key words as signed int64; each state word merges by ops[w] (B2_MERGE_*: ADD wraps modulo
+ * 2^64, MAX is unsigned; a FIRST pair comes from the earliest part holding a nonzero key, the latest when `desc`, and
+ * inside that part from the largest unsigned key, the last such row on ties).  out_keys (n_rows * key_words; 0 for a
+ * NULL single key), out_null (n_rows) and out_acc (n_rows * acc_words) are device buffers with room for n_rows groups;
+ * *n_groups receives the number written.  Runs on `cuda_stream` (0 = legacy default stream) and returns when the result
+ * is there. */
+int32_t b2_agg_merge(int32_t device, uint64_t cuda_stream, uint64_t n_rows, uint32_t key_words, uint32_t acc_words,
+                     const int64_t* keys, uint64_t keys_stride, const uint8_t* key_null, const int64_t* acc, uint64_t acc_stride,
+                     const uint64_t* part_offs, uint32_t n_parts, const uint8_t* ops, int32_t desc,
+                     int64_t* out_keys, uint8_t* out_null, int64_t* out_acc, uint64_t* n_groups);
 
 /* RequestHandler::handle_request for a DAG: run to drain.  Result columns are owned by *out_handle
  * (close it with b2_exec_close). */

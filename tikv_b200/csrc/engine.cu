@@ -2070,6 +2070,67 @@ int32_t b2_exec_agg_word_ops(b2_exec* h, uint8_t* ops, uint32_t* n_inout) {
   return B2_OK;
 }
 
+int32_t b2_agg_merge(int32_t device, uint64_t cuda_stream, uint64_t n_rows, uint32_t key_words, uint32_t acc_words,
+                     const int64_t* keys, uint64_t keys_stride, const uint8_t* key_null, const int64_t* acc, uint64_t acc_stride,
+                     const uint64_t* part_offs, uint32_t n_parts, const uint8_t* ops, int32_t desc,
+                     int64_t* out_keys, uint8_t* out_null, int64_t* out_acc, uint64_t* n_groups) {
+  if (!part_offs || !n_groups || (acc_words && !ops) ||
+      (n_rows && (!keys || !key_null || !out_keys || !out_null || (acc_words && (!acc || !out_acc))))) {
+    g_last_error = "null argument"; return B2_ERR_INVALID_ARG;
+  }
+  if (key_words < 1 || key_words > 4 || n_rows >= (1ull << 31) || n_parts < 1 || part_offs[0] != 0 || part_offs[n_parts] != n_rows ||
+      keys_stride < key_words || (acc_words && acc_stride < acc_words)) {
+    g_last_error = "b2_agg_merge: 1..4 key words, n_rows < 2^31, n_parts >= 1 offsets from 0 to n_rows, row strides >= the words of a row";
+    return B2_ERR_INVALID_ARG;
+  }
+  for (uint32_t p = 0; p < n_parts; ++p)
+    if (part_offs[p] > part_offs[p + 1]) { g_last_error = "b2_agg_merge: part offsets decrease"; return B2_ERR_INVALID_ARG; }
+  for (uint32_t w = 0; w < acc_words; ++w) {
+    const bool pair_ok = ops[w] == B2_MERGE_FIRST_KEY ? w + 1 < acc_words && ops[w + 1] == B2_MERGE_FIRST_VALUE
+                       : ops[w] == B2_MERGE_FIRST_VALUE ? w > 0 && ops[w - 1] == B2_MERGE_FIRST_KEY : ops[w] <= B2_MERGE_XOR;
+    if (!pair_ok) { g_last_error = "b2_agg_merge: unknown op, or a FIRST key word not followed by its value word"; return B2_ERR_INVALID_ARG; }
+  }
+  *n_groups = 0;
+  if (n_rows == 0) return B2_OK;
+  int prev = -1;
+  cudaGetDevice(&prev);
+  if (cudaSetDevice(device) != cudaSuccess) { g_last_error = "cudaSetDevice failed (the CUDA device path is required; there is no CPU fallback)"; return B2_ERR_CUDA; }
+  struct RestoreDevice { int d; ~RestoreDevice() { if (d >= 0) cudaSetDevice(d); } } restore{prev};  // after the buffers below went back
+  const cudaStream_t s = (cudaStream_t)cuda_stream;
+  AggMergeArgs a{};
+  a.keys = (const long long*)keys; a.key_null = key_null; a.acc = (const long long*)acc;
+  a.keys_stride = keys_stride; a.acc_stride = acc_stride; a.n = (uint32_t)n_rows; a.key_words = key_words; a.acc_words = acc_words; a.n_parts = n_parts;
+  a.desc = desc; a.out_keys = (long long*)out_keys; a.out_null = out_null; a.out_acc = (long long*)out_acc;
+  // ops and part offsets travel in one pinned upload; the group count comes back through the same buffer.  Device
+  // buffer: [ops | part offsets] [group count] [scratch of launch_agg_merge], 256-byte aligned
+  const size_t ops_b = (acc_words + 7) & ~7u, offs_b = ((size_t)n_parts + 1) * 8, up_b = ops_b + offs_b;
+  const size_t count_off = (up_b + 255) & ~(size_t)255, scratch_off = count_off + 256;
+  size_t merge_b = 0;
+  cudaError_t e = launch_agg_merge(a, nullptr, &merge_b, s);
+  HostBuf host;
+  DevBuf dev;
+  if (e == cudaSuccess) e = host.reserve(up_b + 8);
+  if (e == cudaSuccess) e = dev.reserve(scratch_off + merge_b);
+  if (e != cudaSuccess) { g_last_error = std::string("b2_agg_merge buffers: ") + cudaGetErrorString(e); return B2_ERR_CUDA; }
+  uint8_t* hp = (uint8_t*)host.p;
+  if (acc_words) memcpy(hp, ops, acc_words);
+  memcpy(hp + ops_b, part_offs, offs_b);
+  uint8_t* dp = (uint8_t*)dev.p;
+  a.ops = dp; a.part_offs = (const unsigned long long*)(dp + ops_b);
+  a.n_groups = (unsigned int*)(dp + count_off);
+  e = cudaMemcpyAsync(dp, hp, up_b, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = launch_agg_merge(a, dp + scratch_off, &merge_b, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(hp + up_b, a.n_groups, 4, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) {
+    cudaStreamSynchronize(s);  // whatever was enqueued still reads the buffers before they go back to the pools
+    g_last_error = std::string("b2_agg_merge: ") + cudaGetErrorString(e);
+    return B2_ERR_CUDA;
+  }
+  *n_groups = *(const unsigned int*)(hp + up_b);
+  return B2_OK;
+}
+
 int32_t b2_dag_handle(const b2_dag_plan* plan, const b2_key_range* ranges, uint32_t n_ranges, const b2_region_source* src,
                       const b2_exec_config* cfg, b2_batch* out, b2_exec** out_handle) {
   b2_exec* h = nullptr;

@@ -196,6 +196,26 @@ struct RawArgs {
   unsigned int* err;              // 1 = a decimal cell does not decode, 2 = heap overflow
 };
 cudaError_t launch_raw_materialise(const RawArgs& R, uint64_t max_rows, cudaStream_t s);
+// Final merge of gathered partial tables (agg_merge.cu, b2_agg_merge): row r = keys[r * keys_stride ..] (key_words
+// words), key_null[r] (NULL mask), acc[r * acc_stride ..] (acc_words state words); ops (acc_words B2_MERGE_*) and
+// part_offs (n_parts + 1 row offsets) are device pointers.  Outputs have room for n groups; *n_groups (device) receives
+// their number.
+struct AggMergeArgs {
+  const long long* keys;
+  const unsigned char* key_null;
+  const long long* acc;
+  uint64_t keys_stride, acc_stride;
+  uint32_t n, key_words, acc_words, n_parts;
+  const unsigned char* ops;
+  const unsigned long long* part_offs;
+  int32_t desc;
+  long long* out_keys;         // n_groups * key_words
+  unsigned char* out_null;     // n_groups
+  long long* out_acc;          // n_groups * acc_words
+  unsigned int* n_groups;
+};
+// cub-style: tmp == nullptr stores the scratch bytes the merge needs in *tmp_bytes and launches nothing
+cudaError_t launch_agg_merge(const AggMergeArgs& a, void* tmp, size_t* tmp_bytes, cudaStream_t s);
 cudaError_t launch_reverse_rows(const unsigned long long* in, const unsigned long long* bm_in, uint64_t in_cap, unsigned long long* out, unsigned long long* bm_out,
                                 uint64_t out_cap, uint64_t n_rows, uint64_t n_take, uint32_t n_cols, cudaStream_t s);
 

@@ -9,7 +9,9 @@ regions on its own GPU; the only exchange is the final merge of those partial re
   TopN             : all_gather of each rank's top-N rows + final selection
   checksum         : all_gather of the u64 partial CRCs + XOR (NCCL has no XOR reduction), all_reduce(SUM) of the counts
 
-All merge functions take plain torch tensors, so they run unchanged on CPU tensors under gloo.
+All merge functions take plain torch tensors, so they run unchanged on CPU tensors under gloo.  The aggregation merge of
+CUDA tensors re-aggregates the gathered rows in one native call (b2_agg_merge: a sort-based group-by on the device that
+gives the torch path's result bit for bit); CPU tensors take that torch path.
 """
 import torch
 import torch.distributed as dist
@@ -83,24 +85,72 @@ def merge_agg_partials(keys, key_null, acc, real_words=(), max_words=(), word_op
     (integer, bit q = q-th expression); the result has the same shapes.
     `max_words` lists the word indices that merge by unsigned maximum (the MAX / MIN extremum keys,
     b2_agg_partials.max_word_mask); every other word is additive: counts, the 32-bit limb sums of integer SUMs and the
-    digits of exact Real SUMs (`real_words` is only for callers that still carry plain f64 words).  Returns (keys, key_null, acc) with one row per group.
+    digits of exact Real SUMs (`real_words` is only for callers that still carry plain f64 words).  Returns (keys, key_null, acc) with one row per group,
+    sorted as torch.unique sorts (NULL mask, key words).
     Integer words are summed exactly (two's-complement wraparound is impossible below 2^32 rows per group).
     `word_ops` (agg_word_ops: one ffi.MERGE_* per word) adds the FIRST / BIT_* states: OR and XOR words reduce with their
     op; a FIRST pair is taken from the earliest gathered part (rank order, the order of shard_blocks' contiguous runs)
-    holding a nonzero key, or the latest when the scan is `desc`; keys are compared only inside one part."""
+    holding a nonzero key, or the latest when the scan is `desc`; keys are compared only inside one part.
+    CUDA tensors merge on the device in one call (b2_agg_merge); CPU tensors and `real_words` merge with torch ops."""
+    multi = keys.dim() == 2
+    kw = keys.shape[1] if multi else 1
+    if keys.is_cuda and not real_words:
+        if _world() == 1:  # nothing to gather: the native merge reads the three tables as they are
+            return _merge_native(keys.view(-1, kw), key_null, acc, [keys.shape[0]], multi, max_words, word_ops, desc)
+        parts = _all_gather_var(torch.cat([keys.view(-1, kw), key_null.to(torch.int64).view(-1, 1), acc], dim=1))
+        allp = torch.cat(parts, dim=0)
+        return _merge_native(allp[:, :kw], allp[:, kw], allp[:, kw + 1:], [p.shape[0] for p in parts], multi, max_words, word_ops, desc)
+    parts = _all_gather_var(torch.cat([keys.view(-1, kw), key_null.to(torch.int64).view(-1, 1), acc], dim=1))
+    return _merge_gathered_torch(parts, kw, multi, real_words, max_words, word_ops, desc)
+
+
+def _merge_native(keys, key_null, acc, part_sizes, multi, max_words=(), word_ops=None, desc=False):
+    """merge_agg_partials on the CUDA device of the rows: b2_agg_merge on the current stream, one call.  keys: int64[n, K]
+    and acc: int64[n, W], rows may be strided (views into gathered rows); key_null: bool or integer NULL masks [n];
+    part_sizes: rows of each gathered part, in rank order."""
+    import ctypes as C
+    from . import ffi
+    if keys.stride(1) != 1:
+        keys = keys.contiguous()
+    if acc.shape[1] and acc.stride(1) != 1:
+        acc = acc.contiguous()
+    if key_null.dtype not in (torch.bool, torch.uint8) or not key_null.is_contiguous():
+        key_null = key_null.to(torch.uint8).contiguous()  # masks are below 2^K <= 16
+    n, kw, aw = keys.shape[0], keys.shape[1], acc.shape[1]
+    ops = list(word_ops) if word_ops is not None else [ffi.MERGE_ADD] * aw
+    for w in max_words:
+        ops[w] = ffi.MERGE_MAX
+    offs = [0]
+    for m in part_sizes:
+        offs.append(offs[-1] + m)
+    out_k = torch.empty((n, kw) if multi else (n,), dtype=torch.int64, device=keys.device)
+    out_n = torch.empty(n, dtype=torch.uint8, device=keys.device)
+    out_a = torch.empty((n, aw), dtype=torch.int64, device=keys.device)
+    ng = C.c_uint64()
+    L = ffi.lib()
+    rc = L.b2_agg_merge(keys.device.index, torch.cuda.current_stream(keys.device).cuda_stream, n, kw, aw,
+                        keys.data_ptr(), keys.stride(0), key_null.data_ptr(), acc.data_ptr(), acc.stride(0) if aw else 0,
+                        (C.c_uint64 * len(offs))(*offs), len(part_sizes), (C.c_uint8 * max(1, aw))(*ops), int(bool(desc)),
+                        out_k.data_ptr(), out_n.data_ptr(), out_a.data_ptr(), C.byref(ng))
+    if rc != 0:
+        raise RuntimeError("b2_agg_merge: " + L.b2_last_error_message().decode())
+    g = ng.value
+    return out_k[:g], (out_n[:g].to(torch.int64) if multi else out_n[:g].view(torch.bool)), out_a[:g]
+
+
+def _merge_gathered_torch(parts, kw, multi, real_words=(), max_words=(), word_ops=None, desc=False):
+    """merge_agg_partials of the gathered rows (kw key words | NULL mask | accumulator words, one tensor per part) with
+    torch ops, on any device: the reference the native merge is tested against."""
     from . import ffi
     ops = list(word_ops) if word_ops is not None else []
     max_words = set(max_words) | {w for w, o in enumerate(ops) if o == ffi.MERGE_MAX}
     bit_words = {w: o for w, o in enumerate(ops) if o in (ffi.MERGE_OR, ffi.MERGE_XOR)}
     first_words = [w for w, o in enumerate(ops) if o == ffi.MERGE_FIRST_KEY]
     special = set(real_words) | max_words | set(bit_words) | {w for w, o in enumerate(ops) if o in (ffi.MERGE_FIRST_KEY, ffi.MERGE_FIRST_VALUE)}
-    multi = keys.dim() == 2
-    kw = keys.shape[1] if multi else 1
-    parts = _all_gather_var(torch.cat([keys.view(-1, kw), key_null.to(torch.int64).view(-1, 1), acc], dim=1))
     part_of = torch.cat([torch.full((p.shape[0],), i, dtype=torch.int64, device=p.device) for i, p in enumerate(parts)])
     allp = torch.cat(parts, dim=0)
     if allp.shape[0] == 0:
-        return keys[:0], key_null[:0], acc[:0]
+        return (allp[:, :kw], allp[:, kw], allp[:, kw + 1:]) if multi else (allp[:, 0], allp[:, 1].bool(), allp[:, 2:])
     k, nul, a = allp[:, :kw], allp[:, kw], allp[:, kw + 1:]
     if not multi:
         k = torch.where(nul.bool().view(-1, 1), torch.zeros_like(k), k)

@@ -177,7 +177,7 @@ JIT_AUTO, JIT_SYNC, JIT_OFF = 0, 1, 2
 EXPORTED_SYMBOLS = [
     "b2_abi_version", "b2_build_info", "b2_last_error_message", "b2_check_supported", "b2_plan_prepare", "b2_plan_precompile", "b2_jit_counters", "b2_plan_literal", "b2_exec_open", "b2_exec_schema",
     "b2_exec_next_batch", "b2_exec_next_batch_async", "b2_exec_poll", "b2_exec_warnings", "b2_region_pin", "b2_region_unpin", "b2_region_cache_stats", "b2_exec_collect_stats", "b2_exec_last_error", "b2_exec_can_be_cached", "b2_exec_encode_batch", "b2_exec_take_scanned_range", "b2_exec_collect_scanned_rows_per_range", "b2_exec_close",
-    "b2_exec_agg_partials", "b2_exec_agg_word_ops", "b2_dag_handle", "b2_checksum_handle", "b2_gen_create", "b2_gen_destroy", "b2_copy_to_host", "b2_copy_to_device",
+    "b2_exec_agg_partials", "b2_exec_agg_word_ops", "b2_agg_merge", "b2_dag_handle", "b2_checksum_handle", "b2_gen_create", "b2_gen_destroy", "b2_copy_to_host", "b2_copy_to_device",
     "b2_sst_decode", "b2_sst_free", "b2_sst_encode",
     "b2_device_count", "b2_host_alloc_pinned", "b2_host_alloc_pinned_near", "b2_device_numa_node", "b2_host_free_pinned",
 ]
@@ -241,6 +241,8 @@ def lib():
     L.b2_exec_agg_partials.restype = i32
     L.b2_exec_agg_word_ops.argtypes = [vp, C.POINTER(C.c_uint8), C.POINTER(u32)]
     L.b2_exec_agg_word_ops.restype = i32
+    L.b2_agg_merge.argtypes = [i32, u64, u64, u32, u32, vp, u64, vp, vp, u64, C.POINTER(u64), u32, C.POINTER(C.c_uint8), i32, vp, vp, vp, C.POINTER(u64)]
+    L.b2_agg_merge.restype = i32
     L.b2_exec_close.argtypes = [vp]
     L.b2_exec_close.restype = None
     L.b2_dag_handle.argtypes = [C.POINTER(DagPlan), C.POINTER(KeyRange), u32, C.POINTER(RegionSource), C.POINTER(ExecConfig), C.POINTER(Batch), C.POINTER(vp)]
