@@ -532,11 +532,18 @@ void b2_region_cache_stats(int32_t device, uint64_t* bytes_cached, uint64_t* hit
  *   5 kLZ4HCCompression     raw LZ4 block format, no frame header): inflated on the device.  A declared size below 4,
  *                           above 255 x the LZ4 bytes or above 1 GiB, or a stream that does not produce exactly that many
  *                           bytes from exactly its bytes, is a corrupted block (B2_ERR_STORAGE)
- *   1, 2, 3, 6, 7, 0x40,    Snappy, zlib, BZip2, Xpress, ZSTD and RocksDB's custom-compressor range: B2_ERR_UNSUPPORTED,
+ *   7 kZSTD,                the contents are  varint32 uncompressed_size | one ZSTD frame (RFC 8878): inflated on the
+ *   0x40 kZSTDNotFinal...   device.  B2_ERR_UNSUPPORTED (the host's reader decides) when the payload does not start with
+ *                           the frame magic 28 B5 2F FD (a skippable or legacy frame) or the frame names a Dictionary_ID.
+ *                           B2_ERR_STORAGE: a declared size below 4 or above 1 GiB, a Frame_Content_Size other than it,
+ *                           a size the frame's block headers cannot produce, anything after the frame, or a frame that
+ *                           does not produce exactly that size (checksum, when present, included)
+ *   1, 2, 3, 6,             Snappy, zlib, BZip2, Xpress and RocksDB's custom-compressor range: B2_ERR_UNSUPPORTED,
  *   0x80 .. 0xfe            a valid block the host's reader may inflate
  *   any other value         (8..0x3f, 0x41..0x7f, 0xff) no RocksDB writer stores it: a corrupted block (B2_ERR_STORAGE)
- * Plain and LZ4 blocks may mix in one run.  Blocks compressed with a dictionary (CompressionOptions::max_dict_bytes > 0)
- * carry no mark of it in the block: the caller must not pass them (TiKV's default sets no dictionary at the LZ4 levels). */
+ * Plain, LZ4 and ZSTD blocks may mix in one run.  Blocks compressed with a dictionary (CompressionOptions::max_dict_bytes
+ * > 0) carry no mark of it in an LZ4 block, nor in a ZSTD frame when the dictionary is raw content (no training: the
+ * frame's Dictionary_ID is 0): the caller must not pass them (TiKV's default sets no dictionary). */
 typedef struct b2_sst_blocks {
   const uint8_t* data;        /* the blocks, back to back or with gaps; host or device memory (see `location`) */
   const uint64_t* block_offs; /* host memory, n_blocks + 1 ascending offsets into data: block b = [block_offs[b], block_offs[b+1])

@@ -10,10 +10,13 @@
 // each bounded by HBM traffic that is a small multiple of the block bytes:
 //   sst_blocks    one thread per data block: the trailer's compression type, the slice; a plain block (type 0) gets its
 //                 contents view (the slice) and its footer read and validated   -> restart points per block; an LZ4 /
-//                 LZ4HC block (type 4 / 5) its framing checked                  -> inflated size per block
+//                 LZ4HC block (type 4 / 5) its framing checked, a ZSTD block (type 7 / 0x40) its frame header and block
+//                 headers walked                                                -> inflated size per block
 //   sst_inflate   only when the run holds LZ4 blocks: one warp per LZ4 block (lz4_block.h) inflates it into the
-//                 handle's inflate buffer at the exclusive sum of the inflated sizes; that is its contents view.  sst_blocks
-//                 then reads the footers of the inflated blocks (the one extra host round trip, for compressed runs only)
+//                 handle's inflate buffer at the exclusive sum of the inflated sizes; that is its contents view.
+//   sst_zstd      only when the run holds ZSTD blocks, beside sst_inflate: one warp per ZSTD block (zstd_block.h, its
+//                 workspace in shared memory) inflates it into the same buffer.  sst_blocks then reads the footers of the
+//                 inflated blocks (the one extra host round trip, for compressed runs only)
 //   sst_count     one thread per restart interval: entries, key bytes, value bytes   -> prefix sums give every
 //                 interval its place in the flat block
 //   sst_expand    one warp per restart interval: the current key lives in the warp's registers (byte j in lane j % 32),
@@ -34,6 +37,7 @@
 
 #include "../../include/b2_copr.h"
 #include "lz4_block.h"
+#include "zstd_block.h"
 
 namespace b2 {
 void set_last_error(const std::string& m);  // engine.cu (thread-local message behind b2_last_error_message)
@@ -86,18 +90,17 @@ __device__ __forceinline__ unsigned int block_restarts(const uint8_t* base, unsi
 
 struct ViewOut { unsigned long long* off; unsigned int* len; };  // the writable side of SstView::voff / vlen
 
-// RocksDB CompressionType values a valid block may carry that are not LZ4's stream format: the built-in Snappy 1, zlib 2,
-// BZip2 3, Xpress 6, ZSTD 7 and 0x40 (kZSTDNotFinalCompression, older files), and the custom-compressor range
-// 0x80..0xfe.  The host's block reader may inflate them: B2_ERR_UNSUPPORTED.  No RocksDB writer stores any other value
+// RocksDB CompressionType values a valid block may carry that the device does not inflate: the built-in Snappy 1, zlib 2,
+// BZip2 3 and Xpress 6, and the custom-compressor range 0x80..0xfe (LZ4 4 / 5 and ZSTD 7 / 0x40 are tested first).  The host's block reader may inflate them: B2_ERR_UNSUPPORTED.  No RocksDB writer stores any other value
 // (8..0x3f, 0x41..0x7f, 0xff kDisableCompressionOption): a block carrying one is damaged.
 __device__ __forceinline__ bool host_compression(unsigned int t) { return (t >= 1 && t <= 7) || t == 0x40 || (t >= 0x80 && t <= 0xfe); }
 
 // Before inflation (inflated == 0): classify every block.  Plain blocks get their contents view and restart count, LZ4
-// blocks their declared size in isz (0 for every other block) and a restart count of 0; their number and the sum of
-// their sizes come back with the first round trip, so the inflate buffer is sized without another.  After inflation:
+// and ZSTD blocks their declared size in isz (0 for every other block) and a restart count of 0; their numbers and the
+// sum of their sizes come back with the first round trip, so the inflate buffer is sized without another.  After inflation:
 // the restart count of every block from its view.
 __global__ void sst_blocks_kernel(SstView S, ViewOut V, unsigned int* nres /* n_blocks + 1, last = 0 */, unsigned long long* isz /* n_blocks + 1 */,
-                                  unsigned int* n_lz4, unsigned long long* lz4_bytes, unsigned int inflated, unsigned int* err) {
+                                  unsigned int* n_lz4, unsigned long long* lz4_bytes, unsigned int* n_zstd, unsigned int inflated, unsigned int* err) {
   const unsigned int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b > S.n_blocks) return;
   if (b == S.n_blocks) { nres[b] = 0; if (!inflated) isz[b] = 0; return; }
@@ -116,6 +119,11 @@ __global__ void sst_blocks_kernel(SstView S, ViewOut V, unsigned int* nres /* n_
       unsigned int n, at;
       if (b2lz4::frame(base, len, &n, &at)) { sz = n; atomicAdd(n_lz4, 1u); atomicAdd(lz4_bytes, sz); }
       else raise(err, SST_CORRUPT);
+    } else if (type == 7 || type == 0x40) {
+      b2zstd::Frame f;
+      const int v = b2zstd::frame(base, len, &f);
+      if (v == b2zstd::kOk) { sz = f.size; atomicAdd(n_zstd, 1u); atomicAdd(lz4_bytes, sz); }
+      else raise(err, v == b2zstd::kUnsupported ? SST_UNSUPPORTED : SST_CORRUPT);
     } else raise(err, host_compression(type) ? SST_UNSUPPORTED : SST_CORRUPT);
   }
   V.off[b] = lo; V.len[b] = vlen;
@@ -130,6 +138,7 @@ __global__ void __launch_bounds__(256) sst_inflate_kernel(SstView S, ViewOut V, 
   if (size == 0) return;
   const uint8_t* base = S.data + S.boffs[b];
   const unsigned int len = (unsigned int)(S.boffs[b + 1] - S.boffs[b]) - S.trailer;
+  if (base[len] != 4 && base[len] != 5) return;  // a ZSTD block: sst_zstd_kernel's
   unsigned int n, p;
   b2lz4::frame(base, len, &n, &p);  // (validated by sst_blocks_kernel: n == size)
   uint8_t* out = (uint8_t*)S.inflated + at;
@@ -137,6 +146,28 @@ __global__ void __launch_bounds__(256) sst_inflate_kernel(SstView S, ViewOut V, 
   if (lane == 0) {
     if (ok) { V.off[b] = kInflated | at; V.len[b] = n; }
     else raise(err, SST_CORRUPT);  // (no view: the footer pass must not read a half-written block and report its garbage)
+  }
+}
+
+// One warp per block: ZSTD blocks inflate into inflated + isz[b] and get that as their view.  Four warps per CTA, each
+// with its workspace (tables and a sequence batch, sizeof(b2zstd::Workspace)) in shared memory.
+constexpr unsigned int kZstdWarps = 4;
+__global__ void __launch_bounds__(32 * kZstdWarps) sst_zstd_kernel(SstView S, ViewOut V, const unsigned long long* isz, unsigned int* err) {
+  __shared__ b2zstd::Workspace ws[kZstdWarps];
+  const unsigned int w = threadIdx.x >> 5, b = blockIdx.x * kZstdWarps + w, lane = threadIdx.x & 31;
+  if (b >= S.n_blocks) return;
+  const unsigned long long at = isz[b];
+  if (isz[b + 1] == at) return;
+  const uint8_t* base = S.data + S.boffs[b];
+  const unsigned int len = (unsigned int)(S.boffs[b + 1] - S.boffs[b]) - S.trailer;
+  if (base[len] != 7 && base[len] != 0x40) return;  // an LZ4 block: sst_inflate_kernel's
+  b2zstd::Frame f;
+  b2zstd::frame(base, len, &f);  // (validated by sst_blocks_kernel: f.size == isz[b + 1] - at)
+  uint8_t* out = (uint8_t*)S.inflated + at;
+  const bool ok = b2zstd::inflate(base, len, f, out, &ws[w], lane, 32);
+  if (lane == 0) {
+    if (ok) { V.off[b] = kInflated | at; V.len[b] = f.size; }
+    else raise(err, SST_CORRUPT);  // (no view, as in sst_inflate_kernel)
   }
 }
 
@@ -443,7 +474,8 @@ int check_err(b2_sst* s, b2_sst& w, const char* what) {
   SST_TRY(cudaStreamSynchronize(s->stream));
   if (code == SST_UNSUPPORTED)
     return sst_fail(B2_ERR_UNSUPPORTED, std::string("b2_sst_decode: ") + what +
-                                            ": a block compressed other than LZ4 / LZ4HC, a data-block hash index or an entry whose value type is not kTypeValue");
+                                            ": a block compressed other than LZ4 / LZ4HC / ZSTD, a ZSTD frame that is not a plain frame without a "
+                                            "dictionary, a data-block hash index or an entry whose value type is not kTypeValue");
   if (code) return sst_fail(B2_ERR_STORAGE, std::string("b2_sst_decode: ") + what + ": corrupted data block");
   return B2_OK;
 }
@@ -465,8 +497,8 @@ int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in,
     if (in->block_offs[b + 1] < in->block_offs[b]) return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_decode: block_offs must ascend");
   const uint64_t lo = nb ? in->block_offs[0] : 0, hi = nb ? in->block_offs[nb] : 0;
   uint64_t h2d = 0;
-  SST_TRY(w.err.reserve(16));
-  SST_TRY(cudaMemsetAsync(w.err.p, 0, 16, s->stream));
+  SST_TRY(w.err.reserve(32));
+  SST_TRY(cudaMemsetAsync(w.err.p, 0, 32, s->stream));
   SST_TRY(w.boffs.reserve(((size_t)nb + 1) * 8));
   std::vector<uint64_t> rel((size_t)nb + 1, 0);
   for (uint32_t b = 0; b <= nb && nb; ++b) rel[b] = in->block_offs[b] - lo;
@@ -489,28 +521,32 @@ int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in,
     S.data = (const uint8_t*)hold.st->buf.p;
   } else S.data = in->data + lo;
   SST_TRY(cudaEventRecord(s->ev0, s->stream));
-  uint32_t n_iv = 0, n_ent = 0, n_lz4 = 0;
+  uint32_t n_iv = 0, n_ent = 0, n_lz4 = 0, n_zstd = 0;
   uint64_t kb = 0, vb = 0;
   if (nb) {
-    unsigned int* err = (unsigned int*)w.err.p;  // [0] error code, [1] LZ4 blocks, [2..3] their inflated bytes (u64)
+    unsigned int* err = (unsigned int*)w.err.p;  // [0] error code, [1] LZ4 blocks, [2..3] LZ4 and ZSTD inflated bytes (u64), [4] ZSTD blocks
     unsigned long long* lz4_bytes = (unsigned long long*)(err + 2);
+    uint32_t counts[4] = {0, 0, 0, 0};  // err[1..4]
     uint64_t total = 0;
     SST_TRY(w.nres.reserve(((size_t)nb + 1) * 4)); SST_TRY(w.isz.reserve(((size_t)nb + 1) * 8));
-    sst_blocks_kernel<<<(nb + 1 + 255) / 256, 256, 0, s->stream>>>(S, V, (unsigned int*)w.nres.p, (unsigned long long*)w.isz.p, err + 1, lz4_bytes, 0, err);
+    sst_blocks_kernel<<<(nb + 1 + 255) / 256, 256, 0, s->stream>>>(S, V, (unsigned int*)w.nres.p, (unsigned long long*)w.isz.p, err + 1, lz4_bytes, err + 4, 0, err);
     if ((rc = scan_inplace(s, w, (unsigned int*)w.nres.p, (size_t)nb + 1))) return rc;
     SST_TRY(cudaMemcpyAsync(&n_iv, (unsigned int*)w.nres.p + nb, 4, cudaMemcpyDeviceToHost, s->stream));
-    SST_TRY(cudaMemcpyAsync(&n_lz4, err + 1, 4, cudaMemcpyDeviceToHost, s->stream));
-    SST_TRY(cudaMemcpyAsync(&total, lz4_bytes, 8, cudaMemcpyDeviceToHost, s->stream));
+    SST_TRY(cudaMemcpyAsync(counts, err + 1, 16, cudaMemcpyDeviceToHost, s->stream));
     if ((rc = check_err(s, w, "block footers"))) return rc;
-    if (n_lz4) {  // inflate the LZ4 blocks, then count the restarts of every block again from the views: one more round trip
+    n_lz4 = counts[0]; n_zstd = counts[3];
+    memcpy(&total, counts + 1, 8);
+    if (n_lz4 || n_zstd) {  // inflate the compressed blocks, then count the restarts of every block again from the views: one more round trip
       if ((rc = scan_inplace(s, w, (unsigned long long*)w.isz.p, (size_t)nb + 1))) return rc;
       SST_TRY(w.inflated.reserve((size_t)total + 16));
       S.inflated = (const uint8_t*)w.inflated.p;
-      sst_inflate_kernel<<<(unsigned int)(((size_t)nb + 7) / 8), 256, 0, s->stream>>>(S, V, (const unsigned long long*)w.isz.p, err);
-      sst_blocks_kernel<<<(nb + 1 + 255) / 256, 256, 0, s->stream>>>(S, V, (unsigned int*)w.nres.p, nullptr, nullptr, nullptr, 1, err);
+      if (n_lz4) sst_inflate_kernel<<<(unsigned int)(((size_t)nb + 7) / 8), 256, 0, s->stream>>>(S, V, (const unsigned long long*)w.isz.p, err);
+      if (n_zstd)
+        sst_zstd_kernel<<<(unsigned int)(((size_t)nb + kZstdWarps - 1) / kZstdWarps), 32 * kZstdWarps, 0, s->stream>>>(S, V, (const unsigned long long*)w.isz.p, err);
+      sst_blocks_kernel<<<(nb + 1 + 255) / 256, 256, 0, s->stream>>>(S, V, (unsigned int*)w.nres.p, nullptr, nullptr, nullptr, nullptr, 1, err);
       if ((rc = scan_inplace(s, w, (unsigned int*)w.nres.p, (size_t)nb + 1))) return rc;
       SST_TRY(cudaMemcpyAsync(&n_iv, (unsigned int*)w.nres.p + nb, 4, cudaMemcpyDeviceToHost, s->stream));
-      if ((rc = check_err(s, w, "LZ4 blocks"))) return rc;
+      if ((rc = check_err(s, w, "compressed blocks"))) return rc;
     }
     if (n_iv >= 0x7ffffff0u) return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_decode: too many restart intervals in one call: pass fewer data blocks");
     SST_TRY(w.cnt_n.reserve(((size_t)n_iv + 1) * 4)); SST_TRY(w.cnt_k.reserve(((size_t)n_iv + 1) * 8)); SST_TRY(w.cnt_v.reserve(((size_t)n_iv + 1) * 8));

@@ -306,7 +306,7 @@ class DeviceRegion:
 
 
 class SstDecoder:
-    """b2_sst_decode: a run of RocksDB data blocks (prefix-compressed keys; stored plain or LZ4 / LZ4HC-compressed, the
+    """b2_sst_decode: a run of RocksDB data blocks (prefix-compressed keys; stored plain, LZ4 / LZ4HC- or ZSTD-compressed, the
     type in each block's trailer) -> a device-resident flat CF block owned by this object.  `data` is a host buffer
     (bytes / numpy uint8 / address) or a device address."""
 
@@ -343,7 +343,7 @@ class SstDecoder:
 
 
 class SstRegion:
-    """A region source whose CF_WRITE blocks arrive as RocksDB data blocks: each (data, block_offs) run, plain or LZ4
+    """A region source whose CF_WRITE blocks arrive as RocksDB data blocks: each (data, block_offs) run, plain, LZ4 or ZSTD
     blocks as stored, is inflated and expanded on the device (b2_sst_decode) and the request reads the decoded blocks
     from HBM.  The other fields follow `like`."""
 
