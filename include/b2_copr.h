@@ -568,6 +568,52 @@ typedef struct b2_sst b2_sst; /* owner of the decoded device block */
  * padded as b2_cf_block requires.  Blocking.  The decoded heaps must stay below 4 GiB each (u32 offsets). */
 int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in, b2_sst** h, b2_cf_block* out, b2_sst_stats* stats);
 void b2_sst_free(b2_sst* h);
+
+/* ---- Sorted runs of one LSM snapshot merged on the device ---------------------------------------------------------
+ * A region that still takes writes keeps its keys in L0 files and several levels, with point tombstones (TiKV's GC
+ * deletes write and default records: MvccTxn::delete_write / delete_value in src/storage/mvcc/txn.rs), rewritten keys (a
+ * commit record over a rollback at the same key) and ingested files (Raft snapshots applied by the raftstore's snapshot
+ * io; imports, components/sst_importer/src/util.rs:213).  b2_sst_merge decodes each run as b2_sst_decode does, keeping the
+ * internal-key footer, and outputs the flat block a RocksDB reader at sequence number `snapshot_seq` sees (DBIter over a
+ * MergingIterator): one entry per user key whose newest visible entry is a value, keys ascending, key_prefix_len and
+ * the footer dropped, padded as b2_cf_block requires and owned by the handle exactly like b2_sst_decode's output.
+ *
+ *   Order       user key bytewise ascending; within one user key the footer seq << 8 | type descending
+ *               (InternalKeyComparator).  Each run ascends strictly in that order (checked: B2_ERR_STORAGE otherwise);
+ *               a run may hold several versions of one key (a compaction under a held snapshot writes them).
+ *   Runs        listed newest first (L0 files newest first, then L1 .. Ln).  That order is used only to break ties: an
+ *               equal (user key, footer) pair in two runs goes to the run listed first.
+ *   Visibility  an entry with seq > snapshot_seq is invisible.  The newest visible entry of a user key decides:
+ *               kTypeValue (1) outputs the key; kTypeDeletion (0) and kTypeSingleDeletion (7) output nothing (DBIter
+ *               treats them alike on reads).  Any other type anywhere in the input (Merge, BlobIndex, ...):
+ *               B2_ERR_UNSUPPORTED, and the host keeps its iterator.
+ *   Global seq  global_seqs[r] != 0 replaces the sequence number of every entry of run r (an ingested file); its stored
+ *               sequence numbers must then be 0 (B2_ERR_STORAGE otherwise).  global_seqs == NULL: every run uses its footers.
+ *   Arguments   (B2_ERR_INVALID_ARG) every run has key_suffix_len == 8 and the first run's key_prefix_len; trailer_len may
+ *               differ per run (block-cache blocks have none, file blocks have one); snapshot_seq and global seqnos
+ *               <= 2^56 - 1; n_runs <= 1024 (0 gives an empty block); each run bounded as in b2_sst_decode, and all
+ *               runs together below 2^31 entries and 4 GiB per decoded heap (footers included).
+ *   Stats       every input entry is counted once: n_in == n_invisible + n_out + n_deletions + n_hidden.
+ *   Not handled range tombstones (the caller checks each file's num_range_deletions or keeps the host path), memtable
+ *               contents and user-defined timestamps.
+ * Blocking.  Device memory of the handle: the decoded runs back to back (decoded bytes + 8 per entry for the footer + 8 per
+ * entry of offsets), two id arrays and three per-entry counters (16 bytes per entry), the largest run's decode buffers
+ * and the output block. */
+typedef struct b2_sst_merge_stats {
+  uint64_t n_in;                 /* entries in all runs */
+  uint64_t n_out;                /* entries written: user keys whose newest visible entry is kTypeValue */
+  uint64_t n_invisible;          /* entries newer than the snapshot */
+  uint64_t n_hidden;             /* visible entries under a newer visible entry of the same user key */
+  uint64_t n_deletions;          /* user keys whose newest visible entry is a deletion */
+  uint64_t key_bytes, val_bytes; /* of the output */
+  uint64_t h2d_bytes;            /* as b2_sst_stats, summed over the runs */
+  float decode_ms, merge_ms;     /* device time (CUDA events): inflate, expansion and staging of every run / ordering, visibility and gather */
+  uint32_t n_lz4_blocks, n_runs;
+} b2_sst_merge_stats;
+int32_t b2_sst_merge(int32_t device, int32_t location, const b2_sst_blocks* runs, uint32_t n_runs,
+                     const uint64_t* global_seqs /* NULL, or n_runs values: 0 = use the footers */, uint64_t snapshot_seq, b2_sst** h,
+                     b2_cf_block* out, b2_sst_merge_stats* stats);
+
 /* tooling (tests / bench): the inverse.  Encodes a device-resident flat block as data blocks of `entries_per_block`
  * entries with a restart point every `restart_interval` entries, key_prefix / internal-key footer (seq 0, kTypeValue)
  * added as asked, 5-byte trailer (type 0, checksum field zero) when trailer_len == 5.  The encoded bytes and the

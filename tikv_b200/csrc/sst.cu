@@ -37,6 +37,7 @@
 
 #include "../../include/b2_copr.h"
 #include "lz4_block.h"
+#include "sst_merge.h"
 #include "zstd_block.h"
 
 namespace b2 {
@@ -320,6 +321,95 @@ __global__ void __launch_bounds__(256) sst_expand_kernel(SstView S, const unsign
   }
 }
 
+// ---- merge of sorted runs (b2_sst_merge; the per-entry rules in sst_merge.h) ----
+struct Flat { const uint8_t* keys; const unsigned int* koff; const uint8_t* vals; const unsigned int* voff; };
+struct Staged { uint8_t* keys; unsigned int* koff; };
+
+// One thread per entry of one decoded run (keys with their footer, already copied to the staged heap at k0): the run's
+// offsets join the staged block at entry n0, the entry is checked against the one before it, and its staged footer
+// becomes the effective one (the global seqno of an ingested run).
+__global__ void sst_stage_kernel(Flat R, unsigned int n, Staged T, unsigned int* tvoff, unsigned int n0, unsigned int k0, unsigned int v0,
+                                 unsigned long long global_seq, unsigned int* err) {
+  const unsigned int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > n) return;
+  T.koff[n0 + i] = k0 + R.koff[i]; tvoff[n0 + i] = v0 + R.voff[i];
+  if (i == n) return;
+  const unsigned int ks = R.koff[i], len = R.koff[i + 1] - ks;
+  const unsigned int ps = i ? R.koff[i - 1] : 0;
+  uint64_t eff;
+  const unsigned int st = b2merge::stage_check(R.keys + ks, len, i ? R.keys + ps : nullptr, ks - ps, global_seq, &eff);
+  if (st) { raise(err, st); return; }
+  uint8_t* f = T.keys + k0 + ks + len - 8;
+#pragma unroll
+  for (int q = 0; q < 8; ++q) f[q] = (uint8_t)(eff >> (8 * q));
+}
+
+__global__ void sst_iota_kernel(unsigned int* ids, unsigned int n) {
+  const unsigned int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) ids[i] = i;
+}
+
+// Internal-key order over staged entry ids; equal internal keys keep the order of their ids, i.e. of the runs as listed.
+struct StagedLess {
+  const uint8_t* keys;
+  const unsigned int* koff;
+  __device__ __forceinline__ bool operator()(unsigned int a, unsigned int b) const {
+    const unsigned int sa = koff[a], sb = koff[b];
+    const int c = b2merge::ikey_cmp(keys + sa, koff[a + 1] - sa, keys + sb, koff[b + 1] - sb);
+    return c ? c < 0 : a < b;
+  }
+};
+
+// One thread per merged position (and one past the end, which zeroes the scans' last element): its verdict, its kept
+// lengths and the stats counters stat[0..2] = invisible, hidden, deleted.
+__global__ void sst_visible_kernel(Staged T, const unsigned int* ids, unsigned int n, unsigned long long snapshot_seq, unsigned int* keep_n,
+                                   unsigned int* keep_k, unsigned int* keep_v, const unsigned int* voff, unsigned long long* stat) {
+  const unsigned int i = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned int v = b2merge::kOut + 10;  // (no position: counts nothing)
+  if (i < n) {
+    const unsigned int id = ids[i], s = T.koff[id], len = T.koff[id + 1] - s, bl = b2merge::body_len(len);
+    const uint64_t f = b2merge::footer_of(T.keys + s + bl, 8);
+    bool same = false;
+    uint64_t pf = 0;
+    if (i) {
+      const unsigned int pid = ids[i - 1], ps = T.koff[pid], pbl = b2merge::body_len(T.koff[pid + 1] - ps);
+      same = b2merge::user_key_cmp(T.keys + ps, pbl, T.keys + s, bl) == 0;
+      pf = b2merge::footer_of(T.keys + ps + pbl, 8);
+    }
+    v = b2merge::verdict(f, same, pf, snapshot_seq);
+    const bool keep = v == b2merge::kOut;
+    keep_n[i] = keep; keep_k[i] = keep ? bl : 0; keep_v[i] = keep ? voff[id + 1] - voff[id] : 0;
+  } else if (i == n) {
+    keep_n[i] = 0; keep_k[i] = 0; keep_v[i] = 0;
+  }
+  const unsigned int mask = __activemask();
+  const unsigned int a = __reduce_add_sync(mask, v == b2merge::kInvisible), h = __reduce_add_sync(mask, v == b2merge::kHidden),
+                     d = __reduce_add_sync(mask, v == b2merge::kDeleted);
+  if ((threadIdx.x & 31) == __ffs(mask) - 1) {
+    if (a) atomicAdd(stat + 0, (unsigned long long)a);
+    if (h) atomicAdd(stat + 1, (unsigned long long)h);
+    if (d) atomicAdd(stat + 2, (unsigned long long)d);
+  }
+}
+
+// One warp per merged position: a kept entry's key body and value leave as consecutive byte stores, as in sst_expand.
+__global__ void __launch_bounds__(256) sst_gather_kernel(Staged T, const unsigned int* tvoff, const uint8_t* tvals, const unsigned int* ids, unsigned int n,
+                                                         const unsigned int* keep_n, const unsigned int* keep_k, const unsigned int* keep_v, FlatOut O) {
+  const unsigned int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (i > n) return;
+  const unsigned int e = keep_n[i], ko = keep_k[i], vo = keep_v[i];
+  if (i == n) { if (lane == 0) { O.koff[e] = ko; O.voff[e] = vo; } return; }
+  if (keep_n[i + 1] == e) return;
+  const unsigned int id = ids[i], kl = keep_k[i + 1] - ko, vl = keep_v[i + 1] - vo;
+  if (lane == 0) { O.koff[e] = ko; O.voff[e] = vo; }
+  const uint8_t* k = T.keys + T.koff[id];
+  const uint8_t* v = tvals + tvoff[id];
+#pragma unroll 1
+  for (unsigned int j = lane; j < kl; j += 32) O.keys[ko + j] = k[j];
+#pragma unroll 1
+  for (unsigned int j = lane; j < vl; j += 32) O.vals[vo + j] = v[j];
+}
+
 // ---- encoder (tooling) ----
 struct FlatIn { const uint8_t* keys; const unsigned int* koff; const uint8_t* vals; const unsigned int* voff; unsigned int n; };
 struct EncOpt { unsigned int per_block, restart, pl, sl, trailer; uint8_t prefix_byte; };
@@ -402,6 +492,20 @@ struct RawBuf {
     if (e == cudaSuccess) cap = n;
     return e;
   }
+  // reserve, keeping the first `used` bytes (the stream's work on them is finished before the old allocation goes)
+  cudaError_t grow(size_t n, size_t used, cudaStream_t st) {
+    if (n <= cap) return cudaSuccess;
+    if (n < 2 * cap) n = 2 * cap;
+    n = (n + 255) & ~(size_t)255;
+    void* q = nullptr;
+    cudaError_t e = cudaMalloc(&q, n);
+    if (e == cudaSuccess && used) e = cudaMemcpyAsync(q, p, used, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { if (q) cudaFree(q); return e; }
+    free();
+    p = q; cap = n;
+    return e;
+  }
   void free() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
 
@@ -410,17 +514,21 @@ struct RawBuf {
 struct b2_sst {
   int device = 0;
   cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;  // ev2 .. ev3: b2_sst_merge's decode and staging
   RawBuf keys, koff, vals, voff;  // decoded block (b2_sst_decode)
   RawBuf enc, enc_offs;           // encoded blocks (b2_sst_encode)
   RawBuf boffs, nres, cnt_n, cnt_k, cnt_v, tmp, err;  // offsets, restart / entry counts and their prefix sums
   RawBuf view_off, view_len, isz, inflated;           // contents views; inflated sizes and bytes of LZ4 blocks
+  RawBuf mkeys, mkoff, mvals, mvoff;                  // b2_sst_merge: every run decoded, back to back, footers kept
+  RawBuf ids0, ids1, keep_n, keep_k, keep_v, mstat;    // merged order (ping-pong), kept counts / lengths, error + stats
   // (the buffers are freed after this, when the handle is deleted: the device is current and the stream drained by then)
   void destroy() {
     cudaSetDevice(device);
     if (stream) cudaStreamSynchronize(stream);
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
+    if (ev2) cudaEventDestroy(ev2);
+    if (ev3) cudaEventDestroy(ev3);
     if (stream) cudaStreamDestroy(stream);
   }
 };
@@ -452,7 +560,8 @@ int sst_handle(int32_t device, b2_sst** h) {
   }
   b2_sst* s = new b2_sst();
   s->device = device;
-  if (cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreate(&s->ev0) != cudaSuccess || cudaEventCreate(&s->ev1) != cudaSuccess) {
+  if (cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreate(&s->ev0) != cudaSuccess || cudaEventCreate(&s->ev1) != cudaSuccess ||
+      cudaEventCreate(&s->ev2) != cudaSuccess || cudaEventCreate(&s->ev3) != cudaSuccess) {
     s->destroy(); delete s;
     return sst_fail(B2_ERR_CUDA, "b2_sst: stream / event creation failed");
   }
@@ -468,33 +577,41 @@ int scan_inplace(b2_sst* s, b2_sst& w, T* a, size_t n) {
   SST_TRY(cub::DeviceScan::ExclusiveSum(w.tmp.p, tb, a, a, (int)n, s->stream));
   return B2_OK;
 }
-int check_err(b2_sst* s, b2_sst& w, const char* what) {
+int check_err(b2_sst* s, b2_sst& w, const char* who, const char* what) {
   unsigned int code = 0;
   SST_TRY(cudaMemcpyAsync(&code, w.err.p, 4, cudaMemcpyDeviceToHost, s->stream));
   SST_TRY(cudaStreamSynchronize(s->stream));
   if (code == SST_UNSUPPORTED)
-    return sst_fail(B2_ERR_UNSUPPORTED, std::string("b2_sst_decode: ") + what +
+    return sst_fail(B2_ERR_UNSUPPORTED, std::string(who) + ": " + what +
                                             ": a block compressed other than LZ4 / LZ4HC / ZSTD, a ZSTD frame that is not a plain frame without a "
                                             "dictionary, a data-block hash index or an entry whose value type is not kTypeValue");
-  if (code) return sst_fail(B2_ERR_STORAGE, std::string("b2_sst_decode: ") + what + ": corrupted data block");
+  if (code) return sst_fail(B2_ERR_STORAGE, std::string(who) + ": " + what + ": corrupted data block");
   return B2_OK;
 }
-}  // namespace
 
-extern "C" {
-
-int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in, b2_sst** hp, b2_cf_block* out, b2_sst_stats* stats) {
-  if (!in || !hp || !out || (location != B2_LOC_HOST && location != B2_LOC_DEVICE) || (in->n_blocks && (!in->data || !in->block_offs)))
-    return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_decode: null argument or bad location");
+int check_blocks_arg(const b2_sst_blocks* in, const char* who) {
+  if ((in->n_blocks && (!in->data || !in->block_offs)))
+    return sst_fail(B2_ERR_INVALID_ARG, std::string(who) + ": null argument or bad location");
   if ((in->trailer_len != 0 && in->trailer_len != 5) || (in->key_suffix_len != 0 && in->key_suffix_len != 8) || in->key_prefix_len > 64 || in->n_blocks >= (1u << 30))
-    return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_decode: trailer_len is 0 or 5, key_suffix_len 0 or 8, key_prefix_len <= 64");
-  int rc = sst_handle(device, hp);
-  if (rc) return rc;
-  b2_sst* s = *hp;
+    return sst_fail(B2_ERR_INVALID_ARG, std::string(who) + ": trailer_len is 0 or 5, key_suffix_len 0 or 8, key_prefix_len <= 64");
+  return B2_OK;
+}
+
+struct Decoded {
+  uint32_t n_ent = 0, n_iv = 0, n_lz4 = 0;
+  uint64_t kb = 0, vb = 0, h2d = 0;
+  float ms = 0.f;  // device time, ev0 .. ev1
+};
+
+// The one decode path: `in` (validated by check_blocks_arg) -> the flat block in the handle's keys / koff / vals / voff,
+// padded as b2_cf_block asks.  `sl` is the footer length dropped from every key: in->key_suffix_len for b2_sst_decode,
+// 0 for b2_sst_merge, which keeps the footer.  Blocking.
+int decode_run(b2_sst* s, int32_t device, int32_t location, const b2_sst_blocks* in, uint32_t sl, const char* who, Decoded* r) {
+  int rc;
   b2_sst& w = *s;
   const uint32_t nb = in->n_blocks;
   for (uint32_t b = 0; b < nb; ++b)
-    if (in->block_offs[b + 1] < in->block_offs[b]) return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_decode: block_offs must ascend");
+    if (in->block_offs[b + 1] < in->block_offs[b]) return sst_fail(B2_ERR_INVALID_ARG, std::string(who) + ": block_offs must ascend");
   const uint64_t lo = nb ? in->block_offs[0] : 0, hi = nb ? in->block_offs[nb] : 0;
   uint64_t h2d = 0;
   SST_TRY(w.err.reserve(32));
@@ -508,7 +625,7 @@ int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in,
   SstView S;
   const ViewOut V{(unsigned long long*)w.view_off.p, (unsigned int*)w.view_len.p};
   S.inflated = nullptr; S.voff = V.off; S.vlen = V.len;
-  S.boffs = (const unsigned long long*)w.boffs.p; S.n_blocks = nb; S.trailer = in->trailer_len; S.pl = in->key_prefix_len; S.sl = in->key_suffix_len;
+  S.boffs = (const unsigned long long*)w.boffs.p; S.n_blocks = nb; S.trailer = in->trailer_len; S.pl = in->key_prefix_len; S.sl = sl;
   struct StagingHold {  // released on every return path
     Staging* st = nullptr;
     ~StagingHold() { if (st) st->mu.unlock(); }
@@ -533,7 +650,7 @@ int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in,
     if ((rc = scan_inplace(s, w, (unsigned int*)w.nres.p, (size_t)nb + 1))) return rc;
     SST_TRY(cudaMemcpyAsync(&n_iv, (unsigned int*)w.nres.p + nb, 4, cudaMemcpyDeviceToHost, s->stream));
     SST_TRY(cudaMemcpyAsync(counts, err + 1, 16, cudaMemcpyDeviceToHost, s->stream));
-    if ((rc = check_err(s, w, "block footers"))) return rc;
+    if ((rc = check_err(s, w, who, "block footers"))) return rc;
     n_lz4 = counts[0]; n_zstd = counts[3];
     memcpy(&total, counts + 1, 8);
     if (n_lz4 || n_zstd) {  // inflate the compressed blocks, then count the restarts of every block again from the views: one more round trip
@@ -546,9 +663,9 @@ int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in,
       sst_blocks_kernel<<<(nb + 1 + 255) / 256, 256, 0, s->stream>>>(S, V, (unsigned int*)w.nres.p, nullptr, nullptr, nullptr, nullptr, 1, err);
       if ((rc = scan_inplace(s, w, (unsigned int*)w.nres.p, (size_t)nb + 1))) return rc;
       SST_TRY(cudaMemcpyAsync(&n_iv, (unsigned int*)w.nres.p + nb, 4, cudaMemcpyDeviceToHost, s->stream));
-      if ((rc = check_err(s, w, "compressed blocks"))) return rc;
+      if ((rc = check_err(s, w, who, "compressed blocks"))) return rc;
     }
-    if (n_iv >= 0x7ffffff0u) return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_decode: too many restart intervals in one call: pass fewer data blocks");
+    if (n_iv >= 0x7ffffff0u) return sst_fail(B2_ERR_INVALID_ARG, std::string(who) + ": too many restart intervals in one call: pass fewer data blocks");
     SST_TRY(w.cnt_n.reserve(((size_t)n_iv + 1) * 4)); SST_TRY(w.cnt_k.reserve(((size_t)n_iv + 1) * 8)); SST_TRY(w.cnt_v.reserve(((size_t)n_iv + 1) * 8));
     sst_count_kernel<<<(n_iv + 1 + 127) / 128, 128, 0, s->stream>>>(S, (const unsigned int*)w.nres.p, n_iv, (unsigned int*)w.cnt_n.p, (unsigned long long*)w.cnt_k.p,
                                                                    (unsigned long long*)w.cnt_v.p, (unsigned int*)w.err.p);
@@ -558,8 +675,8 @@ int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in,
     SST_TRY(cudaMemcpyAsync(&n_ent, (unsigned int*)w.cnt_n.p + n_iv, 4, cudaMemcpyDeviceToHost, s->stream));
     SST_TRY(cudaMemcpyAsync(&kb, (unsigned long long*)w.cnt_k.p + n_iv, 8, cudaMemcpyDeviceToHost, s->stream));
     SST_TRY(cudaMemcpyAsync(&vb, (unsigned long long*)w.cnt_v.p + n_iv, 8, cudaMemcpyDeviceToHost, s->stream));
-    if ((rc = check_err(s, w, "entries"))) return rc;
-    if (kb > 0xfffffff0ull || vb > 0xfffffff0ull) return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_decode: a decoded heap exceeds 4 GiB (u32 offsets): pass fewer data blocks per call");
+    if ((rc = check_err(s, w, who, "entries"))) return rc;
+    if (kb > 0xfffffff0ull || vb > 0xfffffff0ull) return sst_fail(B2_ERR_INVALID_ARG, std::string(who) + ": a decoded heap exceeds 4 GiB (u32 offsets): pass fewer data blocks per call");
   }
   // heaps padded as b2_cf_block asks (16-byte lines + 16 readable bytes past the end)
   SST_TRY(s->keys.reserve(((size_t)kb + 47) & ~(size_t)15)); SST_TRY(s->vals.reserve(((size_t)vb + 47) & ~(size_t)15));
@@ -576,14 +693,152 @@ int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in,
   SST_TRY(cudaMemsetAsync((uint8_t*)s->keys.p + kb, 0, (((size_t)kb + 47) & ~(size_t)15) - kb, s->stream));
   SST_TRY(cudaMemsetAsync((uint8_t*)s->vals.p + vb, 0, (((size_t)vb + 47) & ~(size_t)15) - vb, s->stream));
   SST_TRY(cudaEventRecord(s->ev1, s->stream));
-  if ((rc = check_err(s, w, "entries"))) return rc;
+  if ((rc = check_err(s, w, who, "entries"))) return rc;
+  r->n_ent = n_ent; r->n_iv = n_iv; r->n_lz4 = n_lz4; r->kb = kb; r->vb = vb; r->h2d = h2d;
+  cudaEventElapsedTime(&r->ms, s->ev0, s->ev1);
+  return B2_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int32_t b2_sst_decode(int32_t device, int32_t location, const b2_sst_blocks* in, b2_sst** hp, b2_cf_block* out, b2_sst_stats* stats) {
+  if (!in || !hp || !out || (location != B2_LOC_HOST && location != B2_LOC_DEVICE))
+    return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_decode: null argument or bad location");
+  int rc = check_blocks_arg(in, "b2_sst_decode");
+  if (rc) return rc;
+  if ((rc = sst_handle(device, hp))) return rc;
+  b2_sst* s = *hp;
+  Decoded d;
+  if ((rc = decode_run(s, device, location, in, in->key_suffix_len, "b2_sst_decode", &d))) return rc;
   memset(out, 0, sizeof(*out));
-  out->keys = O.keys; out->key_offs = O.koff; out->vals = O.vals; out->val_offs = O.voff; out->n = n_ent;
+  out->keys = (const uint8_t*)s->keys.p; out->key_offs = (const uint32_t*)s->koff.p; out->vals = (const uint8_t*)s->vals.p; out->val_offs = (const uint32_t*)s->voff.p;
+  out->n = d.n_ent;
   if (stats) {
     memset(stats, 0, sizeof(*stats));
-    stats->n_entries = n_ent; stats->key_bytes = kb; stats->val_bytes = vb; stats->n_restart_intervals = n_iv; stats->h2d_bytes = h2d;
-    stats->n_lz4_blocks = n_lz4;
-    cudaEventElapsedTime(&stats->decode_ms, s->ev0, s->ev1);
+    stats->n_entries = d.n_ent; stats->key_bytes = d.kb; stats->val_bytes = d.vb; stats->n_restart_intervals = d.n_iv; stats->h2d_bytes = d.h2d;
+    stats->n_lz4_blocks = d.n_lz4;
+    stats->decode_ms = d.ms;
+  }
+  return B2_OK;
+}
+
+int32_t b2_sst_merge(int32_t device, int32_t location, const b2_sst_blocks* runs, uint32_t n_runs, const uint64_t* global_seqs, uint64_t snapshot_seq, b2_sst** hp,
+                     b2_cf_block* out, b2_sst_merge_stats* stats) {
+  const char* who = "b2_sst_merge";
+  if (!hp || !out || (n_runs && !runs) || (location != B2_LOC_HOST && location != B2_LOC_DEVICE))
+    return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_merge: null argument or bad location");
+  if (n_runs > 1024 || snapshot_seq > b2merge::kMaxSeq) return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_merge: n_runs <= 1024 and snapshot_seq <= 2^56 - 1");
+  int rc;
+  for (uint32_t r = 0; r < n_runs; ++r) {
+    if ((rc = check_blocks_arg(&runs[r], who))) return rc;
+    if (runs[r].key_suffix_len != 8 || runs[r].key_prefix_len != runs[0].key_prefix_len || (global_seqs && global_seqs[r] > b2merge::kMaxSeq))
+      return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_merge: every run has key_suffix_len 8 and the first run's key_prefix_len; global seqnos <= 2^56 - 1");
+  }
+  if ((rc = sst_handle(device, hp))) return rc;
+  b2_sst* s = *hp;
+  b2_sst& w = *s;
+  // 1. every run decoded with its footers, appended to the staged block (mkeys / mkoff / mvals / mvoff)
+  SST_TRY(w.mstat.reserve(32));  // u64 [0] error code (low word), [1] invisible, [2] hidden, [3] deleted
+  SST_TRY(cudaMemsetAsync(w.mstat.p, 0, 32, s->stream));
+  unsigned int* merr = (unsigned int*)w.mstat.p;
+  std::vector<uint32_t> base(n_runs + 1, 0);
+  uint64_t k0 = 0, v0 = 0, h2d = 0;
+  uint32_t n_lz4 = 0;
+  SST_TRY(cudaEventRecord(s->ev2, s->stream));
+  for (uint32_t r = 0; r < n_runs; ++r) {
+    Decoded d;
+    if ((rc = decode_run(s, device, location, &runs[r], 0, who, &d))) return rc;
+    h2d += d.h2d; n_lz4 += d.n_lz4;
+    const uint64_t n0 = base[r];
+    if (n0 + d.n_ent >= 0x7fffff00ull || k0 + d.kb > 0xfffffff0ull || v0 + d.vb > 0xfffffff0ull)
+      return sst_fail(B2_ERR_INVALID_ARG, "b2_sst_merge: the runs hold more than 2^31 entries or a heap above 4 GiB (u32 offsets): merge fewer blocks per call");
+    // (+16: the footer of a key shorter than 8 bytes, a corrupted run reported after the merge, is read inside the heap)
+    SST_TRY(w.mkeys.grow((size_t)(k0 + d.kb) + 16, (size_t)k0, s->stream)); SST_TRY(w.mvals.grow((size_t)(v0 + d.vb) + 16, (size_t)v0, s->stream));
+    SST_TRY(w.mkoff.grow((size_t)(n0 + d.n_ent + 1) * 4, (size_t)n0 * 4, s->stream)); SST_TRY(w.mvoff.grow((size_t)(n0 + d.n_ent + 1) * 4, (size_t)n0 * 4, s->stream));
+    if (d.kb) SST_TRY(cudaMemcpyAsync((uint8_t*)w.mkeys.p + k0, s->keys.p, (size_t)d.kb, cudaMemcpyDeviceToDevice, s->stream));
+    if (d.vb) SST_TRY(cudaMemcpyAsync((uint8_t*)w.mvals.p + v0, s->vals.p, (size_t)d.vb, cudaMemcpyDeviceToDevice, s->stream));
+    const Flat R{(const uint8_t*)s->keys.p, (const unsigned int*)s->koff.p, (const uint8_t*)s->vals.p, (const unsigned int*)s->voff.p};
+    sst_stage_kernel<<<(d.n_ent + 1 + 255) / 256, 256, 0, s->stream>>>(R, d.n_ent, Staged{(uint8_t*)w.mkeys.p, (unsigned int*)w.mkoff.p}, (unsigned int*)w.mvoff.p,
+                                                                       (unsigned int)n0, (unsigned int)k0, (unsigned int)v0, global_seqs ? global_seqs[r] : 0, merr);
+    SST_TRY(cudaGetLastError());
+    k0 += d.kb; v0 += d.vb; base[r + 1] = (uint32_t)(n0 + d.n_ent);
+  }
+  SST_TRY(cudaEventRecord(s->ev3, s->stream));
+  SST_TRY(cudaEventRecord(s->ev0, s->stream));
+  const uint32_t N = base[n_runs];
+  const Staged T{(uint8_t*)w.mkeys.p, (unsigned int*)w.mkoff.p};
+  // 2. order: ceil(log2 n_runs) rounds of pairwise merges of adjacent segments, ping-ponging between ids0 and ids1
+  SST_TRY(w.ids0.reserve((size_t)N * 4 + 16)); SST_TRY(w.ids1.reserve((size_t)N * 4 + 16));
+  if (N) sst_iota_kernel<<<(N + 255) / 256, 256, 0, s->stream>>>((unsigned int*)w.ids0.p, N);
+  const StagedLess less{T.keys, T.koff};
+  unsigned int* ids = (unsigned int*)w.ids0.p;
+  size_t tmax = 0;
+  for (int run = 0; run < 2; ++run) {  // run 0 sizes the temporary storage of every merge, run 1 merges
+    if (run) SST_TRY(w.tmp.reserve(tmax + 16));
+    std::vector<uint32_t> b = base;
+    unsigned int *src = (unsigned int*)w.ids0.p, *dst = (unsigned int*)w.ids1.p;
+    while (b.size() > 2) {
+      const size_t m = b.size() - 1;
+      std::vector<uint32_t> nb;
+      for (size_t j = 0; j < m; j += 2) {
+        const uint32_t lo = b[j], mid = b[j + 1], hi = j + 1 < m ? b[j + 2] : mid;
+        nb.push_back(lo);
+        if (mid > lo && hi > mid) {
+          size_t tb = run ? w.tmp.cap : 0;
+          SST_TRY(cub::DeviceMerge::MergeKeys(run ? w.tmp.p : nullptr, tb, src + lo, (int)(mid - lo), src + mid, (int)(hi - mid), dst + lo, less, s->stream));
+          if (tb > tmax) tmax = tb;
+        } else if (run && hi > lo) SST_TRY(cudaMemcpyAsync(dst + lo, src + lo, (size_t)(hi - lo) * 4, cudaMemcpyDeviceToDevice, s->stream));
+      }
+      nb.push_back(b[m]);
+      b.swap(nb);
+      std::swap(src, dst);
+    }
+    ids = src;
+  }
+  // 3. visibility: kept counts and lengths, then their exclusive sums
+  SST_TRY(w.keep_n.reserve((size_t)N * 4 + 16)); SST_TRY(w.keep_k.reserve((size_t)N * 4 + 16)); SST_TRY(w.keep_v.reserve((size_t)N * 4 + 16));
+  unsigned int *keep_n = (unsigned int*)w.keep_n.p, *keep_k = (unsigned int*)w.keep_k.p, *keep_v = (unsigned int*)w.keep_v.p;
+  sst_visible_kernel<<<(N + 1 + 255) / 256, 256, 0, s->stream>>>(T, ids, N, snapshot_seq, keep_n, keep_k, keep_v, (const unsigned int*)w.mvoff.p,
+                                                                 (unsigned long long*)w.mstat.p + 1);
+  if ((rc = scan_inplace(s, w, keep_n, (size_t)N + 1))) return rc;
+  if ((rc = scan_inplace(s, w, keep_k, (size_t)N + 1))) return rc;
+  if ((rc = scan_inplace(s, w, keep_v, (size_t)N + 1))) return rc;
+  uint32_t tot[3];
+  uint64_t st[4];
+  SST_TRY(cudaMemcpyAsync(tot, keep_n + N, 4, cudaMemcpyDeviceToHost, s->stream));
+  SST_TRY(cudaMemcpyAsync(tot + 1, keep_k + N, 4, cudaMemcpyDeviceToHost, s->stream));
+  SST_TRY(cudaMemcpyAsync(tot + 2, keep_v + N, 4, cudaMemcpyDeviceToHost, s->stream));
+  SST_TRY(cudaMemcpyAsync(st, w.mstat.p, 32, cudaMemcpyDeviceToHost, s->stream));
+  SST_TRY(cudaStreamSynchronize(s->stream));
+  if ((uint32_t)st[0] == SST_UNSUPPORTED)
+    return sst_fail(B2_ERR_UNSUPPORTED, "b2_sst_merge: an entry whose value type is not kTypeValue, kTypeDeletion or kTypeSingleDeletion (Merge, BlobIndex, ...)");
+  if ((uint32_t)st[0])
+    return sst_fail(B2_ERR_STORAGE, "b2_sst_merge: a run not strictly ascending in internal-key order, a key shorter than its footer, or a stored sequence "
+                                    "number other than 0 in a run with a global seqno");
+  // 4. gather the kept entries into the handle's block, padded as b2_cf_block asks
+  const uint32_t n_out = tot[0];
+  const uint64_t kb = tot[1], vb = tot[2];
+  SST_TRY(s->keys.reserve(((size_t)kb + 47) & ~(size_t)15)); SST_TRY(s->vals.reserve(((size_t)vb + 47) & ~(size_t)15));
+  SST_TRY(s->koff.reserve(((size_t)n_out + 1) * 4 + 16)); SST_TRY(s->voff.reserve(((size_t)n_out + 1) * 4 + 16));
+  FlatOut O;
+  O.keys = (uint8_t*)s->keys.p; O.koff = (unsigned int*)s->koff.p; O.vals = (uint8_t*)s->vals.p; O.voff = (unsigned int*)s->voff.p;
+  sst_gather_kernel<<<(unsigned int)(((size_t)N + 1 + 7) / 8), 256, 0, s->stream>>>(T, (const unsigned int*)w.mvoff.p, (const uint8_t*)w.mvals.p, ids, N, keep_n,
+                                                                                keep_k, keep_v, O);
+  SST_TRY(cudaGetLastError());
+  SST_TRY(cudaMemsetAsync((uint8_t*)s->keys.p + kb, 0, (((size_t)kb + 47) & ~(size_t)15) - kb, s->stream));
+  SST_TRY(cudaMemsetAsync((uint8_t*)s->vals.p + vb, 0, (((size_t)vb + 47) & ~(size_t)15) - vb, s->stream));
+  SST_TRY(cudaEventRecord(s->ev1, s->stream));
+  SST_TRY(cudaStreamSynchronize(s->stream));
+  memset(out, 0, sizeof(*out));
+  out->keys = O.keys; out->key_offs = O.koff; out->vals = O.vals; out->val_offs = O.voff; out->n = n_out;
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->n_in = N; stats->n_out = n_out; stats->n_invisible = st[1]; stats->n_hidden = st[2]; stats->n_deletions = st[3];
+    stats->key_bytes = kb; stats->val_bytes = vb; stats->h2d_bytes = h2d;
+    cudaEventElapsedTime(&stats->decode_ms, s->ev2, s->ev3);
+    cudaEventElapsedTime(&stats->merge_ms, s->ev0, s->ev1);
+    stats->n_lz4_blocks = n_lz4; stats->n_runs = n_runs;
   }
   return B2_OK;
 }

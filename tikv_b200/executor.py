@@ -314,18 +314,40 @@ class SstDecoder:
         self.device, self.h = device, C.c_void_p()
         self._keep = None
 
-    def decode(self, data, block_offs, trailer_len=5, key_prefix_len=1, key_suffix_len=8, location=ffi.LOC_HOST):
-        L = ffi.lib()
+    @staticmethod
+    def _blocks(data, block_offs, trailer_len, key_prefix_len, key_suffix_len, d):
+        """fills the b2_sst_blocks `d`; returns what must stay alive while it is used"""
         offs = np.ascontiguousarray(np.asarray(block_offs, dtype=np.uint64))
         if isinstance(data, (bytes, bytearray)):
             data = np.frombuffer(bytes(data), dtype=np.uint8)
         ptr = data.ctypes.data if isinstance(data, np.ndarray) else int(data)
-        self._keep = (data, offs)
-        d = ffi.SstBlocks()
         d.data, d.block_offs, d.n_blocks = ptr, offs.ctypes.data, len(offs) - 1
         d.trailer_len, d.key_prefix_len, d.key_suffix_len = trailer_len, key_prefix_len, key_suffix_len
+        return data, offs
+
+    def decode(self, data, block_offs, trailer_len=5, key_prefix_len=1, key_suffix_len=8, location=ffi.LOC_HOST):
+        L = ffi.lib()
+        d = ffi.SstBlocks()
+        self._keep = self._blocks(data, block_offs, trailer_len, key_prefix_len, key_suffix_len, d)
         blk, st = ffi.CfBlock(), ffi.SstStats()
         rc = L.b2_sst_decode(self.device, location, C.byref(d), C.byref(self.h), C.byref(blk), C.byref(st))
+        if rc != 0:
+            raise B2Error(rc, L.b2_last_error_message().decode())
+        return blk, st
+
+    def merge(self, runs, snapshot_seq, global_seqs=None, location=ffi.LOC_HOST):
+        """b2_sst_merge: the sorted runs of one LSM snapshot, newest first, each (data, block_offs) or a dict of decode()'s
+        arguments (data, block_offs, trailer_len, key_prefix_len) -> the flat block a reader at `snapshot_seq` sees."""
+        L = ffi.lib()
+        arr = (ffi.SstBlocks * max(len(runs), 1))()
+        keep = []
+        for i, r in enumerate(runs):
+            a = dict(r) if isinstance(r, dict) else dict(data=r[0], block_offs=r[1])
+            keep.append(self._blocks(a["data"], a["block_offs"], a.get("trailer_len", 5), a.get("key_prefix_len", 1), 8, arr[i]))
+        gs = None if global_seqs is None else (C.c_uint64 * max(len(runs), 1))(*global_seqs)
+        self._keep = (keep, arr, gs)
+        blk, st = ffi.CfBlock(), ffi.SstMergeStats()
+        rc = L.b2_sst_merge(self.device, location, arr, len(runs), gs, snapshot_seq, C.byref(self.h), C.byref(blk), C.byref(st))
         if rc != 0:
             raise B2Error(rc, L.b2_last_error_message().decode())
         return blk, st
@@ -345,19 +367,29 @@ class SstDecoder:
 class SstRegion:
     """A region source whose CF_WRITE blocks arrive as RocksDB data blocks: each (data, block_offs) run, plain, LZ4 or ZSTD
     blocks as stored, is inflated and expanded on the device (b2_sst_decode) and the request reads the decoded blocks
-    from HBM.  The other fields follow `like`."""
+    from HBM.  With `snapshot_seq`, `runs` are the sorted runs of one CF_WRITE LSM, newest first, each (data, offs) or
+    (data, offs, global_seq), merged into one write block as a reader at that sequence number sees it (b2_sst_merge).
+    The other fields follow `like`."""
 
-    def __init__(self, like, runs, device=0, **fmt):
-        self._dec = [SstDecoder(device) for _ in runs]
-        self.stats = []
-        arr = (ffi.CfBlock * len(runs))()
-        for i, (data, offs) in enumerate(runs):
-            arr[i], st = self._dec[i].decode(data, offs, **fmt)
-            self.stats.append(st)
+    def __init__(self, like, runs, device=0, snapshot_seq=None, **fmt):
+        if snapshot_seq is None:
+            self._dec = [SstDecoder(device) for _ in runs]
+            self.stats = []
+            arr = (ffi.CfBlock * len(runs))()
+            for i, (data, offs) in enumerate(runs):
+                arr[i], st = self._dec[i].decode(data, offs, **fmt)
+                self.stats.append(st)
+        else:
+            loc = fmt.pop("location", ffi.LOC_HOST)
+            self._dec = [SstDecoder(device)]
+            arr = (ffi.CfBlock * 1)()
+            arr[0], st = self._dec[0].merge([dict(fmt, data=r[0], block_offs=r[1]) for r in runs], snapshot_seq,
+                                            global_seqs=[r[2] if len(r) > 2 else 0 for r in runs], location=loc)
+            self.stats = [st]
         s = ffi.RegionSource()
         C.memmove(C.byref(s), C.byref(like.c), C.sizeof(s))
         s.location, s.device = ffi.LOC_DEVICE, device
-        s.write, s.n_write = arr, len(runs)
+        s.write, s.n_write = arr, len(arr)
         self._w, self._like = arr, like
         if like.c.n_dflt:  # CF_DEFAULT of the model region must live where `location` says
             self._dflt = DeviceRegion(like, device)

@@ -163,6 +163,12 @@ class SstStats(C.Structure):
                 ("h2d_bytes", C.c_uint64), ("decode_ms", C.c_float), ("n_lz4_blocks", C.c_uint32)]
 
 
+class SstMergeStats(C.Structure):
+    _fields_ = [("n_in", C.c_uint64), ("n_out", C.c_uint64), ("n_invisible", C.c_uint64), ("n_hidden", C.c_uint64), ("n_deletions", C.c_uint64),
+                ("key_bytes", C.c_uint64), ("val_bytes", C.c_uint64), ("h2d_bytes", C.c_uint64), ("decode_ms", C.c_float), ("merge_ms", C.c_float),
+                ("n_lz4_blocks", C.c_uint32), ("n_runs", C.c_uint32)]
+
+
 class SstEncoded(C.Structure):
     _fields_ = [("data", C.c_void_p), ("block_offs", C.c_void_p), ("data_len", C.c_uint64), ("n_blocks", C.c_uint32), ("_pad", C.c_uint32)]
 
@@ -178,7 +184,7 @@ EXPORTED_SYMBOLS = [
     "b2_abi_version", "b2_build_info", "b2_last_error_message", "b2_check_supported", "b2_plan_prepare", "b2_plan_precompile", "b2_jit_counters", "b2_plan_literal", "b2_exec_open", "b2_exec_schema",
     "b2_exec_next_batch", "b2_exec_next_batch_async", "b2_exec_poll", "b2_exec_warnings", "b2_region_pin", "b2_region_unpin", "b2_region_cache_stats", "b2_exec_collect_stats", "b2_exec_last_error", "b2_exec_can_be_cached", "b2_exec_encode_batch", "b2_exec_take_scanned_range", "b2_exec_collect_scanned_rows_per_range", "b2_exec_close",
     "b2_exec_agg_partials", "b2_exec_agg_word_ops", "b2_agg_merge", "b2_dag_handle", "b2_checksum_handle", "b2_gen_create", "b2_gen_destroy", "b2_copy_to_host", "b2_copy_to_device",
-    "b2_sst_decode", "b2_sst_free", "b2_sst_encode",
+    "b2_sst_decode", "b2_sst_merge", "b2_sst_free", "b2_sst_encode",
     "b2_device_count", "b2_host_alloc_pinned", "b2_host_alloc_pinned_near", "b2_device_numa_node", "b2_host_free_pinned",
 ]
 
@@ -255,6 +261,8 @@ def lib():
     L.b2_gen_destroy.restype = None
     L.b2_sst_decode.argtypes = [i32, i32, C.POINTER(SstBlocks), C.POINTER(vp), C.POINTER(CfBlock), C.POINTER(SstStats)]
     L.b2_sst_decode.restype = i32
+    L.b2_sst_merge.argtypes = [i32, i32, C.POINTER(SstBlocks), u32, C.POINTER(u64), u64, C.POINTER(vp), C.POINTER(CfBlock), C.POINTER(SstMergeStats)]
+    L.b2_sst_merge.restype = i32
     L.b2_sst_free.argtypes = [vp]
     L.b2_sst_free.restype = None
     L.b2_sst_encode.argtypes = [i32, C.POINTER(CfBlock), u32, u32, u32, C.c_uint8, u32, u32, C.POINTER(vp), C.POINTER(SstEncoded)]
